@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- SDF queries/s of the Points2Surf reconstruction hot path on B200 (BASELINE.json metric).
+"""bench.py -- SDF queries/s of the Points2Surf reconstruction hot path on H100 (BASELINE.json metric).
 
 One "step" = one pass of the hot path over one shape: point cloud -> candidate grid -> per query
 (kNN-300 patch, 1000-point sub-sample, PointNet stacks, |SDF|+sign) -> SDF band of Q queries.
@@ -13,6 +13,9 @@ no data-path collective, like configs[2]).
           SDF band + voxel indices out, copies inside the timed region
   roofline     : the dominant kernel (tensor-core PointNet pass) against MEASURED_PEAKS.json
   cpu_baseline : the oracle port of the reference's CPU path on a bounded sample of the same queries
+
+`--dump-outputs DIR` writes what the last timed step computed (voxel index and SDF of every query of the band) as
+DIR/<name>.npy, so that two builds can be compared output for output on identical inputs.
 
 `--impl reference` times the reference's own CPU algorithm (oracle port: scipy cKDTree + NumPy sampling +
 torch-CPU network, all host threads) on bounded samples of the same workload.
@@ -54,6 +57,8 @@ def parse():
                     help="'sharded': only the shape-sharded job (configs 3 / 5: --model, --shapes_per_gpu, --grid_res), shapes/s")
     ap.add_argument('--shapes_per_gpu', type=int, default=2)
     ap.add_argument('--skip_sharded', action='store_true', help='headline run without the sharded-job / tile-sharded sections')
+    ap.add_argument('--dump-outputs', dest='dump_outputs', default=None, metavar='DIR',
+                    help='write the outputs of the last timed step as DIR/<name>.npy (float32 / float64, at most 64 MB)')
     return ap.parse_args()
 
 
@@ -203,6 +208,26 @@ def calibrate_output_bias(sd, model, device_index):
     return fc4_bias
 
 
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir, last, rank):
+    """The arrays the timed call returned in its last step: `lin` (int32 voxel index of every query, stored as float64,
+    exact) and `sdf` (float32).  A band too large for DUMP_LIMIT_BYTES is written as a fixed, seeded sample of queries,
+    with the sampled positions in `sample_index`.  Rank r > 0 writes into DIR/rank<r>."""
+    lin, sdf = (x.detach().cpu().numpy() for x in last)
+    arrays = {'lin': lin.astype(np.float64), 'sdf': sdf.astype(np.float32)}
+    per_query = sum(a.itemsize for a in arrays.values()) + 8
+    if lin.size * per_query > DUMP_LIMIT_BYTES:
+        idx = np.sort(np.random.RandomState(0).choice(lin.size, DUMP_LIMIT_BYTES // per_query, replace=False))
+        arrays = {k: a[idx] for k, a in arrays.items()}
+        arrays['sample_index'] = idx.astype(np.float64)
+    d = out_dir if rank == 0 else os.path.join(out_dir, 'rank%d' % rank)
+    os.makedirs(d, exist_ok=True)
+    for k, a in arrays.items():
+        np.save(os.path.join(d, k + '.npy'), a)
+
+
 # ----------------------------------------------------------------------------------------------------
 class ClockSampler(threading.Thread):
     def __init__(self, index):
@@ -211,7 +236,7 @@ class ClockSampler(threading.Thread):
 
     def run(self):
         q = 'clocks.sm,clocks.max.sm,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,' \
-            'clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap'
+            'clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap,power.limit,name'
         while not self.stop_flag:
             try:
                 out = subprocess.run(['nvidia-smi', '-i', str(self.index), '--query-gpu=' + q, '--format=csv,noheader,nounits'],
@@ -228,8 +253,10 @@ class ClockSampler(threading.Thread):
         sm = sorted(int(s[0]) for s in self.samples if s[0].isdigit())
         names = ['hw_slowdown', 'hw_thermal_slowdown', 'sw_thermal_slowdown', 'sw_power_cap']
         reasons = [n for j, n in enumerate(names) if any(s[2 + j].lower().startswith('active') for s in self.samples if len(s) > 2 + j)]
-        return {'sm_mhz': sm[len(sm) // 2] if sm else None, 'sm_max_mhz': int(self.samples[0][1]) if self.samples[0][1].isdigit() else None,
-                'reasons': reasons, 'samples': len(self.samples)}
+        s0 = self.samples[0]
+        return {'sm_mhz': sm[len(sm) // 2] if sm else None, 'sm_max_mhz': int(s0[1]) if s0[1].isdigit() else None,
+                'reasons': reasons, 'samples': len(self.samples),
+                'gpu': s0[7] if len(s0) > 7 else None, 'power_limit_w': s0[6] if len(s0) > 6 else None}
 
 
 
@@ -351,7 +378,7 @@ def run_b200(args):
             print(json.dumps({'metric': 'shapes/sec reconstructed at grid_res=%d (marching cubes and mesh gather included)' % args.grid_res,
                               'value': job['shapes_per_s'], 'unit': 'shapes/s', 'n_gpus': world, 'steps': 1, 'warmup': 1,
                               'ms_per_step': job['ms'], 'higher_is_better': True, 'scaling': 'weak', 'vs_baseline': None,
-                              'dtype': 'f16 operands / f32 accumulate (tcgen05)', 'data': 'synthetic', 'config': {'workload': job['workload']},
+                              'dtype': 'f16 operands / f32 accumulate (wgmma)', 'data': 'synthetic', 'config': {'workload': job['workload']},
                               'clocks': sampler.summary(), 'sharded_job': job}))
         if world > 1:
             dist.destroy_process_group()
@@ -386,18 +413,18 @@ def run_b200(args):
         ops.launch_count(reset=True)
         if not host:
             eng.profile_enable(precision == 'tc')
-        total_ms = 0.0
+        total_ms, out = 0.0, None
         for _ in range(steps):
             flush.zero_()
             torch.cuda.synchronize()
             if host:
                 t0 = time.perf_counter()
-                fn()
+                out = fn()
                 total_ms += (time.perf_counter() - t0) * 1e3     # the host call returns after its D2H completed
             else:
                 e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
                 e0.record()
-                fn()
+                out = fn()
                 e1.record()
                 torch.cuda.synchronize()
                 total_ms += e0.elapsed_time(e1)
@@ -406,15 +433,17 @@ def run_b200(args):
         t = torch.tensor([total_ms], dtype=torch.float64, device=dev)
         if world > 1:
             dist.all_reduce(t, op=dist.ReduceOp.MAX)
-        return float(t.item()), launches
+        return float(t.item()), launches, out
 
     try:
         peaks_hbm = json.load(open(os.path.join(ROOT, 'MEASURED_PEAKS.json')))['hbm_gbs']
     except Exception:
-        peaks_hbm = 6576.1   # B200_PROFILING.md fallback (measured copy bandwidth of this pool)
+        peaks_hbm = 3350.0   # H100 SXM data-sheet HBM3 bandwidth (not a measured figure)
     sampler = ClockSampler(local_rank)
     sampler.start()
-    dev_ms, launches = timed(step_dev, args.steps, max(args.warmup, 3))
+    dev_ms, launches, last = timed(step_dev, args.steps, max(args.warmup, 3))
+    if args.dump_outputs and args.steps > 0:
+        dump_outputs(args.dump_outputs, last, rank)
     guard_total = eng.last_guard_count() if precision == 'tc' else 0   # warm-up + timed steps
 
     prof = eng.profile_get() if precision == 'tc' else None
@@ -490,7 +519,7 @@ def run_b200(args):
             eng_fit.close()
         except Exception as e:  # noqa: BLE001
             tile_sharded = {'error': '%s: %s' % (type(e).__name__, e)}
-    e2e_ms, _ = timed(step_host, args.steps, 1, host=True)
+    e2e_ms, _, _ = timed(step_host, args.steps, 1, host=True)
     guard_frac = guard_total / max(Q * (args.steps + max(args.warmup, 3)), 1)
 
     q_total = torch.tensor([Q], dtype=torch.float64, device=dev)
@@ -508,12 +537,12 @@ def run_b200(args):
             pass
         roofline = None
         if prof and prof['launches'] > 0:
-            peak = peaks.get('bf16_tflops_sustained') or 1400.0
+            peak = peaks.get('bf16_tflops_sustained') or 989.0
             ach = prof['flops'] / (prof['ms'] * 1e-3) / 1e12
             traffic = None   # per-launch DRAM bytes come from an `ncu --set full` capture (profiles/), not from this run
             roofline = {'bound': 'tensor', 'kernel': prof['kernel'], 'achieved': ach, 'peak': peak, 'unit': 'TFLOP/s',
                         'frac': ach / peak, 'traffic': traffic,
-                        'peak_source': 'MEASURED_PEAKS.json bf16_tflops_sustained (of measured)' if peaks else 'fallback 1.4 PFLOP/s sustained (of fallback)',
+                        'peak_source': 'MEASURED_PEAKS.json bf16_tflops_sustained (of measured)' if peaks else 'H100 SXM data sheet, 989 TFLOP/s dense fp16 (not measured)',
                         'flops_per_launch': prof['flops'] / prof['launches'], 'ms_per_launch': prof['ms'] / prof['launches'],
                         'share_of_step': prof['ms'] / dev_ms}
         if args.cpu_sample > 0 and world == 1:
@@ -525,7 +554,7 @@ def run_b200(args):
             'metric': 'SDF queries/sec at grid_res=%d' % args.grid_res, 'value': value, 'unit': 'queries/s',
             'n_gpus': world, 'steps': args.steps, 'warmup': max(args.warmup, 3), 'ms_per_step': dev_ms / args.steps,
             'higher_is_better': True, 'scaling': 'weak', 'vs_baseline': None,
-            'dtype': 'f16 operands / f32 accumulate (tcgen05); hi/lo split f16 (fp32-level) for FC tails and guard-band recompute' if precision == 'tc' else 'f32',
+            'dtype': 'f16 operands / f32 accumulate (wgmma); hi/lo split f16 (fp32-level) for FC tails and guard-band recompute' if precision == 'tc' else 'f32',
             'data': 'synthetic', 'config': dict(workload_config(args, Q), precision=precision, guard_band=guard,
                                                 guard_recompute_fraction=guard_frac),
             'e2e': {'value': e2e_value, 'unit': 'queries/s', 'h2d_bytes_per_step': int(cloud.nbytes), 'd2h_bytes_per_step': int(Q * 8)},

@@ -1,5 +1,5 @@
 /*
- * p2s_b200.h -- C ABI of libp2s_b200.so, the B200 (sm_100a) implementation of the Points2Surf
+ * p2s_b200.h -- C ABI of libp2s_b200.so, the H100 (sm_90a) implementation of the Points2Surf
  * SDF-inference hot path (SURVEY.md section 8).  Plain pointers and sizes only; no torch types.
  *
  * The reference (ErlerPhilipp/points2surf) is pure Python, so "the FFI a maintainer would bind" is
@@ -71,7 +71,7 @@ void p2s_model_destroy(p2s_model* m);
 
 /* Arithmetic of the per-point MLP stacks:
  *   P2S_PRECISION_FP32  CUDA-core fp32 FMA everywhere (accuracy path; also the guard-band recompute path)
- *   P2S_PRECISION_TC    tcgen05 tensor cores, fp16 operands (11-bit significand, same as the TF32 the
+ *   P2S_PRECISION_TC    wgmma tensor cores,  fp16 operands (11-bit significand, same as the TF32 the
  *                       reference's cuDNN Conv1d uses on Ampere+), fp32 accumulate; queries whose
  *                       |sign logit| < guard_band are recomputed on the fp32 path. */
 #define P2S_PRECISION_FP32 0

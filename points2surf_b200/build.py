@@ -1,4 +1,4 @@
-"""Build libp2s_b200.so in-tree with nvcc for sm_100a (no torch dependency, no JIT cache).
+"""Build libp2s_b200.so in-tree with nvcc for sm_90a (H100) (no torch dependency, no JIT cache).
 
     python -m points2surf_b200.build            # incremental
     python -m points2surf_b200.build --force
@@ -13,7 +13,7 @@ CSRC = os.path.join(HERE, 'csrc')
 OBJ = os.path.join(CSRC, 'build')
 LIB = os.path.join(HERE, 'libp2s_b200.so')
 NVCC = os.environ.get('NVCC', '/usr/local/cuda/bin/nvcc')
-FLAGS = ['-O3', '-std=c++17', '-gencode', 'arch=compute_100a,code=sm_100a', '-lineinfo',
+FLAGS = ['-O3', '-std=c++17', '-gencode', 'arch=compute_90a,code=sm_90a', '-lineinfo',
          '-Xcompiler', '-fPIC', '--expt-relaxed-constexpr', '--extended-lambda', '-Xptxas', '-v']
 
 

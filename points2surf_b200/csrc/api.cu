@@ -223,7 +223,7 @@ int p2s_model_create(const p2s_model_config* cfg, const float* blob_host, size_t
         P2S_CUDA(cudaSetDevice(device));
         cudaDeviceProp prop;
         P2S_CUDA(cudaGetDeviceProperties(&prop, device));
-        if (prop.major != 10) throw Error(std::string("libp2s_b200 is built for sm_100a (B200) only; found ") + prop.name);
+        if (prop.major != 9 || prop.minor != 0) throw Error(std::string("libp2s_b200 is built for sm_90a (H100) only; found ") + prop.name);
         Model* m = new Model();
         m->cfg = *cfg;
         m->device = device;

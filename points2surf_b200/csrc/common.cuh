@@ -1,4 +1,4 @@
-// Shared helpers for libp2s_b200.so (sm_100a only).
+// Shared helpers for libp2s_b200.so (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <cstdint>

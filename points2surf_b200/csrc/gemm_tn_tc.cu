@@ -1,14 +1,15 @@
 // Tensor-core weight-gradient GEMM of the training step (SURVEY.md section 8a row a14):
 //     C[N][K] += sum_m A[m][n] * B[m][k]          (dW = dZ^T X; A = dZ [M,N], B = X [M,K], both fp32 row-major)
 // The contraction runs over the rows m (up to 1.3 M of them), so both operands are "transposed" with respect to the
-// K-major layout tcgen05 wants.  The producers do the transposition on the fly: a warp reads whole rows (coalesced),
+// K-major layout wgmma wants.  The producers do the transposition on the fly: a warp reads whole rows (coalesced),
 // every thread ends up with an 8 (m) x 4 (n) block and writes four 16-byte core-matrix rows of the K-major operand
 // image (k = m), split into fp16 hi / lo parts; three MMAs per k-step (lo*hi + hi*lo + hi*hi) keep fp32-level accuracy
 // (same scheme as fc_tc.cu).  One CTA = one 128 (n) x 128 (k) output tile x one slice of the rows; partial tiles are
 // added to C with fp32 atomics (C is zeroed or holds the running gradient).
-//   warps 0-3   A-operand producers (dZ tile 32 rows x 128 n), afterwards the epilogue (TMEM -> atomicAdd)
+//   warps 0-3   A-operand producers (dZ tile 32 rows x 128 n)
 //   warps 4-7   B-operand producers (X tile 32 rows x 128 k)
-//   warp  8     tcgen05.mma issue (elect-one), commits free the stage
+//   warps 8-11  consumer warpgroup 0: wgmma for n rows 0-63 of the tile, then its epilogue (registers -> atomicAdd)
+//   warps 12-15 consumer warpgroup 1: n rows 64-127
 // HBM-bound by design: every dZ element is read once per k-tile (K <= 128: once), X once per n-tile (L2 hits).
 #include "model.cuh"
 #include "tc_ptx.cuh"
@@ -26,8 +27,7 @@ constexpr uint32_t kStageOp = 2 * kHalf;       // hi + lo
 constexpr uint32_t kSmem = kStages * 2 * kStageOp + 256;
 
 struct Bars {
-    uint64_t full[kStages], empty[kStages], d_full;
-    uint32_t tmem_base;
+    uint64_t full[kStages], empty[kStages];
 };
 
 // Fill one operand image (hi | lo) from src[m][c0 .. c0+127] (row stride ld), rows m0 .. m0+31 (< m_end), cols < ncols.
@@ -65,7 +65,7 @@ __device__ __forceinline__ void fill_operand(uint8_t* dst, const float* __restri
     }
 }
 
-__global__ void __launch_bounds__(288)
+__global__ void __launch_bounds__(512, 1)
 gemm_tn_tc_kernel(const float* __restrict__ A, int lda, const float* __restrict__ B, int ldb, float* __restrict__ C, int ldc,
                   int64_t M, int N, int K, int64_t rows_per_split) {
     extern __shared__ __align__(1024) uint8_t smem[];
@@ -76,15 +76,10 @@ gemm_tn_tc_kernel(const float* __restrict__ A, int lda, const float* __restrict_
     const int64_t m_end = m_begin + rows_per_split < M ? m_begin + rows_per_split : M;
     const int nsteps = (int)((m_end - m_begin + kBM - 1) / kBM);
     if (tid == 0) {
-        for (int s = 0; s < kStages; ++s) { mbar_init(&bars->full[s], 256); mbar_init(&bars->empty[s], 1); }
-        mbar_init(&bars->d_full, 1);
+        for (int s = 0; s < kStages; ++s) { mbar_init(&bars->full[s], 256); mbar_init(&bars->empty[s], 2); }
         fence_mbar_init();
     }
-    if (warp == 8) { tmem_alloc(&bars->tmem_base, 128); tmem_relinquish(); }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = bars->tmem_base;
     uint8_t* opA = smem;                                  // [stage][hi | lo]
     uint8_t* opB = smem + kStages * kStageOp;
 
@@ -101,51 +96,45 @@ gemm_tn_tc_kernel(const float* __restrict__ A, int lda, const float* __restrict_
             fence_proxy_async_smem();
             mbar_arrive(&bars->full[s]);
         }
-        if (isA) {
-            // ---- epilogue: TMEM lane = n row of the tile
-            mbar_wait_bounded(&bars->d_full, 0);
-            tc_fence_after();
-            const int n = n0 + warp * 32 + (tid & 31);
-            const uint32_t lane_base = (uint32_t)(warp * 32) << 16;
-#pragma unroll
-            for (int c0 = 0; c0 < 128; c0 += 32) {
-                uint32_t r[32];
-                tmem_ld_x32(tmem + lane_base + c0, r);
-                tmem_ld_wait();
-                if (n < N) {
-#pragma unroll
-                    for (int j = 0; j < 32; ++j)
-                        if (k0 + c0 + j < K) atomicAdd(C + (int64_t)n * ldc + k0 + c0 + j, __uint_as_float(r[j]));
-                }
-            }
-        }
     } else {
-        const uint32_t idesc = make_idesc_f16(128, 128);
-        const uint64_t dsc_a = make_smem_desc(smem_u32(opA), 128, 512);
+        const int wg = (warp - 8) >> 2, t = tid & 127;
+        const uint64_t dsc_a = make_smem_desc(smem_u32(opA) + (uint32_t)wg * 4096u, 128, 512);
         const uint64_t dsc_b = make_smem_desc(smem_u32(opB), 128, 512);
+        float acc[64];
+#pragma unroll
+        for (int i = 0; i < 64; ++i) acc[i] = 0.f;
         for (int st = 0; st < nsteps; ++st) {
             const int s = st % kStages;
-            const uint32_t use = (uint32_t)(st / kStages);
-            mbar_wait_bounded(&bars->full[s], use & 1);
-            tc_fence_after();
-            if (elect_one()) {
-                const uint64_t a_hi = dsc_a + (uint64_t)(s * (kStageOp >> 4)), a_lo = a_hi + (uint64_t)(kHalf >> 4);
-                const uint64_t b_hi = dsc_b + (uint64_t)(s * (kStageOp >> 4)), b_lo = b_hi + (uint64_t)(kHalf >> 4);
+            mbar_wait_bounded(&bars->full[s], (uint32_t)(st / kStages) & 1);
+            const uint64_t a_hi = dsc_a + (uint64_t)(s * (kStageOp >> 4)), a_lo = a_hi + (uint64_t)(kHalf >> 4);
+            const uint64_t b_hi = dsc_b + (uint64_t)(s * (kStageOp >> 4)), b_lo = b_hi + (uint64_t)(kHalf >> 4);
+            wgmma_fence();
 #pragma unroll
-                for (int ks = 0; ks < kBM / 16; ++ks) {
-                    mma_ss(tmem, a_lo + (uint64_t)(ks * 16), b_hi + (uint64_t)(ks * 16), idesc, (st | ks) > 0);
-                    mma_ss(tmem, a_hi + (uint64_t)(ks * 16), b_lo + (uint64_t)(ks * 16), idesc, 1);
-                    mma_ss(tmem, a_hi + (uint64_t)(ks * 16), b_hi + (uint64_t)(ks * 16), idesc, 1);
-                }
-                mma_commit(&bars->empty[s]);
-                if (st == nsteps - 1) mma_commit(&bars->d_full);
+            for (int ks = 0; ks < kBM / 16; ++ks) {
+                wgmma_ss_n128(acc, a_lo + (uint64_t)(ks * 16), b_hi + (uint64_t)(ks * 16), (st | ks) > 0);
+                wgmma_ss_n128(acc, a_hi + (uint64_t)(ks * 16), b_lo + (uint64_t)(ks * 16), 1);
+                wgmma_ss_n128(acc, a_hi + (uint64_t)(ks * 16), b_hi + (uint64_t)(ks * 16), 1);
             }
-            __syncwarp();
+            wgmma_commit();
+            wgmma_wait<1>();                               // step st - 1 has finished reading its stage
+            if (st >= 1 && t == 0) mbar_arrive(&bars->empty[(st - 1) % kStages]);
+        }
+        wgmma_wait<0>();
+        fence_regs(acc);
+        if (nsteps == 0) return;
+        // ---- epilogue: thread holds n rows r, r + 8 and k column pairs 8 j + 2 (t % 4) of the tile
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int n = n0 + wg * 64 + (t >> 5) * 16 + ((t & 31) >> 2) + h * 8;
+            if (n >= N) continue;
+#pragma unroll
+            for (int j = 0; j < 16; ++j) {
+                const int k = k0 + 8 * j + 2 * (t & 3);
+                if (k < K) atomicAdd(C + (int64_t)n * ldc + k, acc[4 * j + 2 * h]);
+                if (k + 1 < K) atomicAdd(C + (int64_t)n * ldc + k + 1, acc[4 * j + 2 * h + 1]);
+            }
         }
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 8) tmem_dealloc(tmem, 128);
 }
 
 }  // namespace
@@ -168,7 +157,7 @@ void launch_gemm_tn_tc(const float* A, int lda, const float* B, int ldb, float* 
         P2S_CUDA(cudaFuncSetAttribute(gemm_tn_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmem));
         attr = true;
     }
-    int dev = 0, sms = 148;
+    int dev = 0, sms = 132;
     P2S_CUDA(cudaGetDevice(&dev));
     P2S_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
     const int64_t tiles = cdiv(N, 128) * cdiv(K, 128);
@@ -178,7 +167,7 @@ void launch_gemm_tn_tc(const float* A, int lda, const float* B, int ldb, float* 
     int64_t rows = cdiv(cdiv(M, splits), kBM) * kBM;
     splits = cdiv(M, rows);
     dim3 grid((unsigned)cdiv(N, 128), (unsigned)cdiv(K, 128), (unsigned)splits);
-    P2S_LAUNCH(gemm_tn_tc_kernel, grid, 288, kSmem, st, A, lda, B, ldb, C, ldc, M, N, K, rows);
+    P2S_LAUNCH(gemm_tn_tc_kernel, grid, 512, kSmem, st, A, lda, B, ldb, C, ldc, M, N, K, rows);
 }
 
 }  // namespace p2s

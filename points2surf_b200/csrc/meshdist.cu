@@ -8,7 +8,7 @@
 //   3. exhaustive tiled nearest neighbour: every CTA stages a slab of the target cloud in shared memory, one source
 //   point per thread, best (d^2, index) merged across slabs with a 64-bit atomicMin
 //   4. finalise: sqrt, sum (f64) and max per direction.
-// 10^4 x 10^4 samples = 10^8 distance evaluations: compute-trivial, latency-bound; sized to fill the 148 SMs.
+// 10^4 x 10^4 samples = 10^8 distance evaluations: compute-trivial, latency-bound; sized to fill the SMs (132 on an H100).
 #include "common.cuh"
 #include <cub/device/device_scan.cuh>
 
@@ -143,7 +143,7 @@ void nn_core(const float* a, int64_t na, const float* b, int64_t nb, float* dist
     auto& sc = scratch();
     unsigned long long* best = sc.best.as<unsigned long long>((size_t)na);
     P2S_LAUNCH(nn_init_kernel, (unsigned)cdiv(na, 256), 256, 0, st, best, na);
-    int dev = 0, sms = 148;
+    int dev = 0, sms = 132;
     P2S_CUDA(cudaGetDevice(&dev));
     P2S_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
     int64_t gx = cdiv(na, kNnThreads);

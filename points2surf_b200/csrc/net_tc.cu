@@ -1,7 +1,7 @@
-// Tensor-core implementation of PointsToSurfModel.forward (source/points_to_surf_model.py:296-352) for sm_100a.
+// Tensor-core implementation of PointsToSurfModel.forward (source/points_to_surf_model.py:296-352) for sm_90a.
 //
-// The per-point Conv1d(k=1) stacks (98 % of the FLOPs, SURVEY.md section 2a) run as tcgen05.mma tiles with fp16
-// operands / fp32 accumulation in TMEM; the three dependent max-reductions of the vanilla network become three
+// The per-point Conv1d(k=1) stacks (98 % of the FLOPs, SURVEY.md section 2a) run as wgmma tiles with fp16
+// operands / fp32 accumulation in registers; the three dependent max-reductions of the vanilla network become three
 // launches of ONE kernel (`pointnet_pass_kernel`):
 //   pass A  QSTN        : x(1300 pts) -> 64 (fp32 FMA) -> 128 -> 1024, max          (model.py:100-107)
 //   pass B  STN64       : x -> 64 -> 64 | 64 -> 128 -> 1024, max                     (model.py:190-191,41-48)
@@ -9,25 +9,20 @@
 // The quaternion rotation is folded into the first layer's weights per query (W0*R), the 64x64 feature
 // transform into conv1's weights per query (W1*T), both exactly as in the fp32 path up to operation order.
 //
-// Tile = 128 points of one query (segments are padded with a duplicate of their first point: max-invariant).
-// Mid layers: M = 128 points (TMEM lanes), A operand = activations in TMEM (tcgen05.st by the epilogue
-// warps), B operand = weights in smem.  Big layer 128 -> 1024: M = 128 channels, A = resident W3 tile in smem,
-// B = the tile's 128-channel activations in smem, D[channel lane][point column] so that the max over points is
-// a per-thread reduction over TMEM columns (no shuffles).  Each CTA owns 512 of the 1024 channels (its half
-// of W3, 128 KB fp16, stays resident in shared memory); CTA 2j and 2j+1 stream the same queries.
+// Tile = 64 points of one query (segments are padded with a duplicate of their first point: max-invariant).
+// Mid layers: M = 64 points, A operand = activations in registers (the accumulator fragment of one layer, packed to
+// fp16 pairs, is the A fragment of the next), B operand = weights in smem.  Big layer 128 -> 1024: M = 64 channels,
+// A = resident W3 block in smem, B = the tile's 128-channel activations in smem, D[channel][point] so that the max
+// over points is a per-thread reduction over accumulator columns (the 4 lanes sharing a row are combined once per
+// query).  Each CTA owns 512 of the 1024 channels (its half of W3, 128 KB fp16, stays resident in shared memory);
+// CTA 2j and 2j+1 stream the same queries.
 //
-// Warp roles (576 threads): warps 14-17 compute the first layer (fp32 FMA) of every tile; warps 0-3 and 9-12 are two
-// chains (even / odd tiles) running the mid-layer epilogues (thread = point = TMEM lane); warps 4-7 the column-max
-// epilogue of the big layer; warp 8 issues the big-layer MMAs (blocking waits), warp 13 the mid-layer MMAs of both
-// chains (polling).
+// Each warpgroup of the CTA streams its own queries (qi = wg, wg + 2, ...) through all layers; the two warpgroups
+// interleave on the SM, so one's FMA / epilogue work overlaps the other's tensor-core work.
 //
-// The small per-query FC tails between the passes run as fp32 FMA GEMMs (net_fp32.cu kernels).
+// The small per-query FC tails between the passes run on the split-precision FC kernel (fc_tc.cu).
 #include "model.cuh"
 #include "tc_ptx.cuh"
-
-#ifndef P2S_TC_BOUNDED_WAIT
-#define P2S_TC_BOUNDED_WAIT 1   // trap instead of hanging if a barrier protocol bug slips in
-#endif
 
 namespace p2s {
 
@@ -35,39 +30,37 @@ using namespace ptx;
 
 namespace {
 
-constexpr int kTile = 128;
-constexpr int kThreads = 576;   // warps 0-3 chain 0 | 4-7 column-max epilogue | 8 big-layer issuer | 9-12 chain 1 | 13 mid-layer issuer | 14-17 first layer
+constexpr int kTile = 64;                       // points per tile (M of the mid layers, N of the big layer)
+constexpr int kWG = 2;                          // warpgroups per CTA
+constexpr int kThreads = 128 * kWG;
+constexpr uint32_t kAct2Bytes = kTile * 128 * 2;   // 64 points x 128 channels fp16
 // shared memory map (bytes).  PRECISE = split-precision variant used for the guard-band recompute: every fp16
 // operand x is carried as x_hi + x_lo and every product is evaluated as a_hi*b_hi + a_lo*b_hi + a_hi*b_lo (three MMAs
 // per k-step, ~2^-22 relative), so the images are twice as large and a CTA owns one 128-channel chunk instead of four.
-constexpr uint32_t kAct2Bytes = 32768;                   // 128 points x 128 channels fp16
-constexpr uint32_t kSmallBytes = 192 * 4 + 320 * 4 + 168;  // Wq[3][64], biases[256 mid + 64 first], barriers
 template <bool PRECISE>
 struct Cfg {
     static constexpr int kChunks = PRECISE ? 1 : 4;                  // 128-channel chunks of the big layer per CTA
     static constexpr int kSplit = 8 / kChunks;                       // CTAs that share one query stream
     static constexpr uint32_t kChunkBytes = PRECISE ? 65536u : 32768u;   // W3 chunk image (hi [+ lo])
     static constexpr uint32_t kW3Bytes = kChunks * kChunkBytes;
-    static constexpr uint32_t kMidBytes = (8192u + 8192u + 16384u) * (PRECISE ? 2u : 1u);
-    static constexpr uint32_t kOffMid = kW3Bytes;
-    static constexpr uint32_t kOffAct2 = kOffMid + kMidBytes;
-    static constexpr uint32_t kOffSmall = kOffAct2 + 2 * kAct2Bytes;   // normal: two tile buffers; precise: one buffer, hi | lo
-    static constexpr uint32_t kSmemBytes = kOffSmall + kSmallBytes;
-    static constexpr uint32_t kACols = PRECISE ? 64u : 32u;          // TMEM columns of one chain's A operand (hi [+ lo])
-    static constexpr uint32_t kPerqBytes = PRECISE ? 16384u : 8192u; // per-query conv1*(T+I) image
     static constexpr uint32_t kMidScale = PRECISE ? 2u : 1u;
+    static constexpr uint32_t kMidBytes = (8192u + 8192u + 16384u) * kMidScale;
+    static constexpr uint32_t kPerqBytes = PRECISE ? 16384u : 8192u; // per-query conv1*(T+I) image
+    static constexpr uint32_t kOffMid = kW3Bytes;
+    // per warpgroup: the big layer's B operand (hi [| lo]), the per-query conv1 image, (W0*R)^T [3][64] fp32
+    static constexpr uint32_t kWgPerq = kAct2Bytes * kMidScale;
+    static constexpr uint32_t kWgWq = kWgPerq + kPerqBytes;
+    static constexpr uint32_t kWgBytes = kWgWq + 192 * 4;
+    static constexpr uint32_t kOffWg = kOffMid + kMidBytes;
+    static constexpr uint32_t kOffBias = kOffWg + kWG * kWgBytes;     // [256] mid biases back to back, [64] first-layer bias
+    static constexpr uint32_t kSmemBytes = kOffBias + 320 * 4;
 };
 static_assert(Cfg<false>::kSmemBytes <= 232448 && Cfg<true>::kSmemBytes <= 232448, "shared memory budget");
-// TMEM map (columns)
-constexpr uint32_t kColD3 = 0;      // 2 stages x 128
-constexpr uint32_t kColDmid = 256;  // 128 columns: accumulator of the 128-channel mid layers (shared by the chains)
-constexpr uint32_t kColDmidB = 448; // 64 columns: accumulator of the 64-channel mid layers (shared by the chains)
-constexpr uint32_t kColA = 384;     // 2 chains x 32 (fp16 pairs, K = 64)
 
 struct Seg {
     const float* ptr;   // [B, n, 3]
     int n;              // real points per query
-    int tiles;          // ceil(n / 128)
+    int tiles;          // ceil(n / kTile)
     int center;         // subtract the query point (model.py:303)
 };
 
@@ -79,7 +72,7 @@ struct PassParams {
     int B;
     const float* W0;           // [64,3]
     const float* b0;           // [64]
-    int num_mid;               // 1 or 3
+    int num_mid;               // 1 or 3: 64 -> 128, or 64 -> 64 -> 64 -> 128
     int mid_N[3];              // output channels of each mid layer
     const uint8_t* mid_img[3]; // packed fp16 operand images (K-major, LBO 128, SBO 1024)
     const float* mid_bias[3];
@@ -87,41 +80,7 @@ struct PassParams {
     const uint8_t* perq_img;   // [B] x 8192 B (precise: hi | lo, 16384 B)
     const uint8_t* w3_img;     // [8 chunks][32768 B] (precise: [8][hi | lo])  (K-major, LBO 128, SBO 2048)
     float* out;                // [B,1024] raw max (bias / ReLU applied by the consumer: the FC kernel's producers add it on load)
-    long long* wstats;         // diagnostics: per-role barrier wait cycles (null = off)
 };
-
-struct Bars {
-    uint64_t w_full, wq_full, perq_done;
-    uint64_t dmid_free[2];      // [0]: 128-column accumulator, [1]: 64-column accumulator
-    uint64_t a_ready[2], a_free[2], dmid_ready[2];
-    uint64_t act2_full[2], act2_empty[2], d3_full[2], d3_empty[2];
-    uint32_t tmem_base;
-};
-static_assert(sizeof(Bars) <= 168, "barrier block");
-
-// `acc` (diagnostics, P2S_TC_WAITSTATS=1): cycles this thread spent waiting are added to it
-__device__ __forceinline__ void wait_bar(uint64_t* bar, uint32_t parity, long long* acc = nullptr) {
-#if P2S_TC_BOUNDED_WAIT
-    long long t0 = clock64();
-    while (!mbar_try_wait(bar, parity)) {
-        if (clock64() - t0 > 2000000000LL) {
-            printf("p2s: mbarrier timeout block %d thread %d bar %p parity %u\n", blockIdx.x, threadIdx.x, (void*)bar, parity);
-            __trap();
-        }
-    }
-    if (acc) *acc += clock64() - t0;
-#else
-    mbar_wait(bar, parity);
-#endif
-}
-// wait statistics layout: [role 0..5][slot 0..7]; roles: 0 big-layer issuer, 1 mid issuer, 2 chain 0, 3 chain 1, 4 first layer,
-// 5 column-max epilogue; slots: 0 act2_full, 1 d3_empty, 2 dmid_free, 3 dmid_ready, 4 act2_empty, 5 a_free, 6 d3_full, 7 role cycles
-enum { WS_ACT2_FULL = 0, WS_D3_EMPTY, WS_DMID_FREE, WS_DMID_READY, WS_ACT2_EMPTY, WS_A_FREE, WS_D3_FULL, WS_TOTAL, WS_SLOTS };
-__device__ __forceinline__ void ws_flush(long long* g, int role, const long long* ws, long long t_begin) {
-    if (!g || (threadIdx.x & 31) != 0) return;
-    for (int i = 0; i < WS_TOTAL; ++i) if (ws[i]) atomicAdd((unsigned long long*)&g[role * WS_SLOTS + i], (unsigned long long)ws[i]);
-    atomicAdd((unsigned long long*)&g[role * WS_SLOTS + WS_TOTAL], (unsigned long long)(clock64() - t_begin));
-}
 
 // relu(a), relu(b) -> packed fp16x2 (low half = a), saturating
 __device__ __forceinline__ uint32_t pack_relu(float a, float b) {
@@ -135,40 +94,56 @@ __device__ __forceinline__ void pack_relu_split(float a, float b, uint32_t& hi, 
     const float2 hf = __half22float2(*reinterpret_cast<const __half2*>(&hi));
     lo = pack_half2(fmaxf(a, 0.f) - hf.x, fmaxf(b, 0.f) - hf.y);
 }
+template <bool PRECISE>
+__device__ __forceinline__ void pack_act(float a, float b, uint32_t& hi, uint32_t& lo) {
+    if (PRECISE) pack_relu_split(a, b, hi, lo);
+    else hi = pack_relu(a, b);
+}
 
-template <bool PRECISE, bool STATS = false>
+// one k16 step of a mid layer: D (+)= A (registers) * W^T; precise: a_lo*w_hi + a_hi*w_lo + a_hi*w_hi (small terms first)
+template <bool PRECISE, int R>
+__device__ __forceinline__ void mid_mma(float (&d)[R], const uint32_t (&a)[4], const uint32_t (&al)[4], uint64_t w, uint64_t w_lo, uint32_t acc) {
+    if (R == 32) {
+        auto& d32 = reinterpret_cast<float (&)[32]>(d);
+        if (PRECISE) { wgmma_rs_n64(d32, al, w, acc); wgmma_rs_n64(d32, a, w_lo, 1); wgmma_rs_n64(d32, a, w, 1); }
+        else wgmma_rs_n64(d32, a, w, acc);
+    } else {
+        auto& d64 = reinterpret_cast<float (&)[64]>(d);
+        if (PRECISE) { wgmma_rs_n128(d64, al, w, acc); wgmma_rs_n128(d64, a, w_lo, 1); wgmma_rs_n128(d64, a, w, 1); }
+        else wgmma_rs_n128(d64, a, w, acc);
+    }
+}
+
+template <bool PRECISE>
 __global__ void __launch_bounds__(kThreads, 1) pointnet_pass_kernel(const PassParams p) {
     using C = Cfg<PRECISE>;
-    constexpr uint32_t kOffMid = C::kOffMid, kOffAct2 = C::kOffAct2, kOffSmall = C::kOffSmall, kOffW3 = 0;
+    constexpr int kL = PRECISE ? 4 : 1;
     extern __shared__ __align__(1024) uint8_t smem[];
-    float* s_wq = reinterpret_cast<float*>(smem + kOffSmall);             // [3][64]: rows of (W0*R)^T
-    float* s_bias = s_wq + 192;                                           // [256] mid biases back to back, [64] first-layer bias
-    Bars* bars = reinterpret_cast<Bars*>(s_bias + 320);
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    float* s_bias = reinterpret_cast<float*>(smem + C::kOffBias);
+    const int tid = threadIdx.x, wg = tid >> 7, t = tid & 127, lane = tid & 31, q4 = lane & 3;
+    const int r0 = (t >> 5) * 16 + (lane >> 2);                          // fragment rows r0, r0 + 8
     const int part = blockIdx.x % C::kSplit;                             // which 128-channel chunks this CTA owns
     const int stream = blockIdx.x / C::kSplit, nstreams = gridDim.x / C::kSplit;
     const int nq = (p.B > stream) ? (p.B - stream + nstreams - 1) / nstreams : 0;   // queries of this CTA
     const int tpq = p.tiles_per_query;
-    const int ntiles = nq * tpq;
-
-    if (tid == 0) {
-        mbar_init(&bars->w_full, 1);
-        mbar_init(&bars->wq_full, 1);
-        mbar_init(&bars->perq_done, 1);
-        mbar_init(&bars->dmid_free[0], 128);
-        mbar_init(&bars->dmid_free[1], 128);
-        for (int i = 0; i < 2; ++i) {
-            mbar_init(&bars->a_ready[i], 128);
-            mbar_init(&bars->a_free[i], 128);
-            mbar_init(&bars->dmid_ready[i], 1);
-            mbar_init(&bars->act2_full[i], 128);
-            mbar_init(&bars->act2_empty[i], 1);
-            mbar_init(&bars->d3_full[i], 1);
-            mbar_init(&bars->d3_empty[i], 128);
-        }
-        fence_mbar_init();
+    uint32_t mid_off[3] = {0, 0, 0};
+    {
+        uint32_t o = 0;
+        for (int l = 0; l < p.num_mid; ++l) { mid_off[l] = o; o += (uint32_t)p.mid_N[l] * 128u * C::kMidScale; }
     }
-    if (warp == 8) { tmem_alloc(&bars->tmem_base, 512); tmem_relinquish(); }
+
+    // ---- resident weights: this CTA's W3 chunks, the mid layers shared by every query, the biases
+    if (nq > 0) {
+        const uint4* src = reinterpret_cast<const uint4*>(p.w3_img + (size_t)part * C::kW3Bytes);
+        uint4* dst = reinterpret_cast<uint4*>(smem);
+        for (uint32_t i = tid; i < C::kW3Bytes / 16; i += kThreads) dst[i] = src[i];
+        for (int l = 0; l < p.num_mid; ++l) {
+            if (l == p.perq_layer) continue;
+            const uint4* s = reinterpret_cast<const uint4*>(p.mid_img[l]);
+            uint4* d = reinterpret_cast<uint4*>(smem + C::kOffMid + mid_off[l]);
+            for (uint32_t i = tid; i < (uint32_t)p.mid_N[l] * 8u * C::kMidScale; i += kThreads) d[i] = s[i];
+        }
+    }
     {
         int off = 0;
         for (int l = 0; l < p.num_mid; ++l) {
@@ -177,366 +152,181 @@ __global__ void __launch_bounds__(kThreads, 1) pointnet_pass_kernel(const PassPa
         }
         for (int i = tid; i < 64; i += kThreads) s_bias[256 + i] = p.b0[i];
     }
-    tc_fence_before();
+    fence_proxy_async_smem();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = bars->tmem_base;
-    long long ws[WS_TOTAL] = {0, 0, 0, 0, 0, 0, 0};
-    long long* const wsp = STATS ? ws : nullptr;            // STATS = false: everything below folds away
-    const long long t_begin = STATS ? clock64() : 0;
 
-    if (warp == 8) {
-        // =============================================================== big-layer MMA issuer (+ resident weight loads)
-        // The whole warp runs the warp-uniform loop; one elected lane issues the asynchronous instructions.
-        if (ntiles > 0) {
-            if (lane == 0) {
-                uint32_t bytes = C::kW3Bytes;
-                for (int l = 0; l < p.num_mid; ++l) if (l != p.perq_layer) bytes += (uint32_t)p.mid_N[l] * 128u * C::kMidScale;
-                mbar_arrive_expect_tx(&bars->w_full, bytes);
-                for (uint32_t o = 0; o < C::kW3Bytes; o += 32768u)
-                    bulk_g2s(smem + kOffW3 + o, p.w3_img + (size_t)part * C::kW3Bytes + o, 32768, &bars->w_full);
-                uint32_t o = 0;
-                for (int l = 0; l < p.num_mid; ++l) {
-                    const uint32_t lb = (uint32_t)p.mid_N[l] * 128u * C::kMidScale;
-                    if (l != p.perq_layer) bulk_g2s(smem + kOffMid + o, p.mid_img[l], lb, &bars->w_full);
-                    else {
-                        mbar_arrive_expect_tx(&bars->wq_full, C::kPerqBytes);
-                        bulk_g2s(smem + kOffMid + o, p.perq_img + (size_t)stream * C::kPerqBytes, C::kPerqBytes, &bars->wq_full);
-                    }
-                    o += lb;
-                }
+    uint8_t* wsm = smem + C::kOffWg + wg * C::kWgBytes;
+    uint8_t* act2 = wsm;                                                  // [point][channel] K-major, LBO 128, SBO 2048
+    uint8_t* perq = wsm + C::kWgPerq;
+    float* wq = reinterpret_cast<float*>(wsm + C::kWgWq);                 // [3][64]: rows of (W0*R)^T
+    const float* s_b0 = s_bias + 256;
+    const uint32_t bar_id = 1 + (uint32_t)wg;
+    auto wg_sync = [&]() { asm volatile("bar.sync %0, 128;" ::"r"(bar_id) : "memory"); };
+    const uint64_t dsc_act2 = make_smem_desc(smem_u32(act2), 128, 2048);
+    const uint64_t dsc_w3 = make_smem_desc(smem_u32(smem), 128, 2048);
+    uint64_t dsc_mid[3], dsc_mid_lo[3];
+    for (int l = 0; l < 3; ++l) {
+        const bool pq = l == p.perq_layer;
+        dsc_mid[l] = make_smem_desc(pq ? smem_u32(perq) : smem_u32(smem + C::kOffMid) + mid_off[l], 128, 1024);
+        dsc_mid_lo[l] = dsc_mid[l] + (uint64_t)((pq ? 8192u : (uint32_t)p.mid_N[l] * 128u) >> 4);   // lo image follows hi
+    }
+
+    for (int qi = wg; qi < nq; qi += kWG) {
+        const size_t q = (size_t)stream + (size_t)qi * nstreams;
+        wg_sync();                                    // the previous query's readers of wq / perq are done
+        if (t < 64) {
+            // (W0 * R)^T for this query
+            const float w0 = p.W0[t * 3 + 0], w1 = p.W0[t * 3 + 1], w2 = p.W0[t * 3 + 2];
+            float r[9] = {1.f, 0.f, 0.f, 0.f, 1.f, 0.f, 0.f, 0.f, 1.f};
+            if (p.R) {
+#pragma unroll
+                for (int i = 0; i < 9; ++i) r[i] = p.R[q * 9 + i];
             }
-            __syncwarp();
-            wait_bar(&bars->w_full, 0);
-            const uint32_t idesc_l3 = make_idesc_f16(128, 128);
-            const uint64_t dsc_w3 = make_smem_desc(smem_u32(smem + kOffW3), 128, 2048);
-            const uint64_t dsc_act2 = make_smem_desc(smem_u32(smem + kOffAct2), 128, 2048);
-            for (int it = 0; it < ntiles; ++it) {
-                // normal: tile t uses activation buffer t & 1; precise: one buffer (hi | lo) used by every tile
-                const uint32_t buf = PRECISE ? 0u : ((uint32_t)it & 1), buse = PRECISE ? (uint32_t)it : ((uint32_t)it >> 1);
-                wait_bar(&bars->act2_full[buf], buse & 1, wsp ? wsp + WS_ACT2_FULL : nullptr);
-                const uint64_t db = dsc_act2 + (uint64_t)(buf * (kAct2Bytes >> 4));
-#pragma unroll
-                for (int c = 0; c < C::kChunks; ++c) {
-                    const uint32_t g = (uint32_t)(it * C::kChunks + c);
-                    const uint32_t stage = g & 1, use = g >> 1;
-                    wait_bar(&bars->d3_empty[stage], (use & 1) ^ 1, wsp ? wsp + WS_D3_EMPTY : nullptr);
-                    tc_fence_after();
-                    if (elect_one()) {
-                        const uint64_t da = dsc_w3 + (uint64_t)((uint32_t)c * (C::kChunkBytes >> 4));
-                        const uint32_t d = tmem + kColD3 + stage * 128u;
-                        if (PRECISE) {
-                            const uint64_t da_lo = da + (uint64_t)(32768u >> 4), db_lo = db + (uint64_t)(32768u >> 4);
-#pragma unroll
-                            for (int ks = 0; ks < 8; ++ks) {
-                                mma_ss(d, da_lo + (uint64_t)(ks * 16), db + (uint64_t)(ks * 16), idesc_l3, ks > 0);   // small terms first
-                                mma_ss(d, da + (uint64_t)(ks * 16), db_lo + (uint64_t)(ks * 16), idesc_l3, 1);
-                                mma_ss(d, da + (uint64_t)(ks * 16), db + (uint64_t)(ks * 16), idesc_l3, 1);
-                            }
-                        } else {
-#pragma unroll
-                            for (int ks = 0; ks < 8; ++ks)
-                                mma_ss(d, da + (uint64_t)(ks * 16), db + (uint64_t)(ks * 16), idesc_l3, ks > 0);
-                        }
-                        mma_commit(&bars->d3_full[stage]);
-                        if (c == C::kChunks - 1) mma_commit(&bars->act2_empty[buf]);
-                    }
-                    __syncwarp();
-                }
-            }
+            wq[0 * 64 + t] = w0 * r[0] + w1 * r[3] + w2 * r[6];
+            wq[1 * 64 + t] = w0 * r[1] + w1 * r[4] + w2 * r[7];
+            wq[2 * 64 + t] = w0 * r[2] + w1 * r[5] + w2 * r[8];
         }
-    } else if (warp == 13) {
-        // =============================================================== mid-layer MMA issuer (serves the two chains)
-        if (ntiles > 0) {
-            uint32_t mid_off[3] = {0, 0, 0};
-            {
-                uint32_t o = 0;
-                for (int l = 0; l < p.num_mid; ++l) { mid_off[l] = o; o += (uint32_t)p.mid_N[l] * 128u * C::kMidScale; }
+        if (p.perq_layer >= 0) {
+            const uint4* s = reinterpret_cast<const uint4*>(p.perq_img + q * C::kPerqBytes);
+            uint4* d = reinterpret_cast<uint4*>(perq);
+            for (uint32_t i = t; i < C::kPerqBytes / 16; i += 128) d[i] = s[i];
+            fence_proxy_async_smem();
+        }
+        wg_sync();
+        float rmax[4 * C::kChunks];                   // [chunk][64-channel block][row r0 | r0 + 8]
+#pragma unroll
+        for (int i = 0; i < 4 * C::kChunks; ++i) rmax[i] = -INFINITY;
+        for (int tq = 0; tq < tpq; ++tq) {
+            // ---- first layer (fp32 FMA): points r0, r0 + 8 of the tile, channels 16 kk + 8 hc + 2 q4 + {0, 1}
+            const int sgi = tq < p.seg[0].tiles ? 0 : 1;
+            const Seg& sg = p.seg[sgi];
+            float cx = 0.f, cy = 0.f, cz = 0.f;
+            if (sg.center) { cx = p.query[q * 3 + 0]; cy = p.query[q * 3 + 1]; cz = p.query[q * 3 + 2]; }
+            float px[2], py[2], pz[2];
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                int local = (tq - (sgi ? p.seg[0].tiles : 0)) * kTile + r0 + 8 * h;
+                if (local >= sg.n) local = 0;                              // duplicate padding
+                const float* src = sg.ptr + (q * sg.n + local) * 3;
+                px[h] = src[0] - cx; py[h] = src[1] - cy; pz[h] = src[2] - cz;   // model.py:303
             }
-            const bool perq = p.perq_layer >= 0;
-            wait_bar(&bars->w_full, 0);
-            if (perq) wait_bar(&bars->wq_full, 0);
-            const uint64_t dsc_mid0 = make_smem_desc(smem_u32(smem + kOffMid) + mid_off[0], 128, 1024);
-            const uint64_t dsc_mid1 = make_smem_desc(smem_u32(smem + kOffMid) + mid_off[1], 128, 1024);
-            const uint64_t dsc_mid2 = make_smem_desc(smem_u32(smem + kOffMid) + mid_off[2], 128, 1024);
-            const uint32_t idesc_mid0 = make_idesc_f16(128, (uint32_t)p.mid_N[0]);
-            const uint32_t idesc_mid1 = make_idesc_f16(128, (uint32_t)(p.num_mid > 1 ? p.mid_N[1] : 64));
-            const uint32_t idesc_mid2 = make_idesc_f16(128, (uint32_t)(p.num_mid > 2 ? p.mid_N[2] : 64));
-            int it_mid0 = 0, it_mid1 = 1, l_mid0 = 0, l_mid1 = 0;
-            uint32_t rnd0 = 0, rnd1 = 0;        // per-chain (tile, layer) round counter
-            uint32_t g_mid = 0;                 // mid MMAs issued so far (alternates which chain is polled first)
-            uint32_t g_buf0 = 0, g_buf1 = 0;    // MMAs issued into the 128-column / 64-column accumulator
-            int loaded_q = 0, perq_count = 0;   // per-query weights resident for local query `loaded_q`
-            bool pq_loading = false;
-            while (it_mid0 < ntiles || it_mid1 < ntiles) {
-                // ---- per-query weight prefetch: once every tile of the resident query has issued its MMA
-                if (perq) {
-                    if (!pq_loading && perq_count == tpq && loaded_q + 1 < nq && mbar_test_wait_warp(&bars->perq_done, (uint32_t)loaded_q & 1)) {
-                        if (elect_one()) {
-                            mbar_arrive_expect_tx(&bars->wq_full, C::kPerqBytes);
-                            bulk_g2s(smem + kOffMid + mid_off[p.perq_layer],
-                                     p.perq_img + ((size_t)stream + (size_t)(loaded_q + 1) * nstreams) * C::kPerqBytes, C::kPerqBytes, &bars->wq_full);
-                        }
-                        __syncwarp();
-                        pq_loading = true;
-                    }
-                    if (pq_loading && mbar_test_wait_warp(&bars->wq_full, (uint32_t)(loaded_q + 1) & 1)) {
-                        ++loaded_q; perq_count = 0; pq_loading = false;
+            uint32_t a[4][4], al[4][kL];
+#pragma unroll
+            for (int kk = 0; kk < 4; ++kk) {
+#pragma unroll
+                for (int hc = 0; hc < 2; ++hc) {
+                    const int ch = kk * 16 + hc * 8 + 2 * q4;
+                    const float2 wx = *reinterpret_cast<const float2*>(wq + 0 * 64 + ch);
+                    const float2 wy = *reinterpret_cast<const float2*>(wq + 1 * 64 + ch);
+                    const float2 wz = *reinterpret_cast<const float2*>(wq + 2 * 64 + ch);
+                    const float2 bb = *reinterpret_cast<const float2*>(s_b0 + ch);
+#pragma unroll
+                    for (int h = 0; h < 2; ++h) {
+                        // same association as the fp32 path: fma(wx, x, fma(wy, y, fma(wz, z, b)))
+                        const float v0 = fmaf(wx.x, px[h], fmaf(wy.x, py[h], fmaf(wz.x, pz[h], bb.x)));
+                        const float v1 = fmaf(wx.y, px[h], fmaf(wy.y, py[h], fmaf(wz.y, pz[h], bb.y)));
+                        pack_act<PRECISE>(v0, v1, a[kk][hc * 2 + h], al[kk][PRECISE ? hc * 2 + h : 0]);
                     }
                 }
-                auto try_mid = [&](const int c, int& it_m, int& l_m, uint32_t& rn) {
-                    if (it_m >= ntiles) return;
-                    const int l = l_m;
-                    if (l == p.perq_layer && it_m / tpq != loaded_q) return;
-                    if (!mbar_test_wait_warp(&bars->a_ready[c], rn & 1)) return;
-                    const bool small = !PRECISE && (p.mid_N[l] == 64);   // precise: the A operands occupy the small accumulator's columns
-                    uint32_t& g_buf = small ? g_buf1 : g_buf0;
-                    if (g_buf > 0) wait_bar(&bars->dmid_free[small ? 1 : 0], (g_buf - 1) & 1, wsp ? wsp + WS_DMID_FREE : nullptr);   // short: the previous read-out
-                    tc_fence_after();
-                    const uint32_t idesc = l == 0 ? idesc_mid0 : (l == 1 ? idesc_mid1 : idesc_mid2);
-                    const uint64_t dsc = l == 0 ? dsc_mid0 : (l == 1 ? dsc_mid1 : dsc_mid2);
-                    const uint32_t a_t = tmem + kColA + (uint32_t)c * C::kACols;
-                    const uint32_t d_t = tmem + (small ? kColDmidB : kColDmid);
-                    const bool pq_last = (l == p.perq_layer) && (perq_count + 1 == tpq);
-                    if (elect_one()) {
-                        if (PRECISE) {
-                            const uint64_t dsc_lo = dsc + (uint64_t)(((uint32_t)p.mid_N[l] * 128u) >> 4);   // lo image follows hi
-#pragma unroll
-                            for (int ks = 0; ks < 4; ++ks) {
-                                mma_ts(d_t, a_t + 32 + ks * 8, dsc + (uint64_t)(ks * 16), idesc, ks > 0);     // a_lo * b_hi
-                                mma_ts(d_t, a_t + ks * 8, dsc_lo + (uint64_t)(ks * 16), idesc, 1);          // a_hi * b_lo
-                                mma_ts(d_t, a_t + ks * 8, dsc + (uint64_t)(ks * 16), idesc, 1);             // a_hi * b_hi
-                            }
-                        } else {
-#pragma unroll
-                            for (int ks = 0; ks < 4; ++ks)
-                                mma_ts(d_t, a_t + ks * 8, dsc + (uint64_t)(ks * 16), idesc, ks > 0);
-                        }
-                        mma_commit(&bars->dmid_ready[c]);
-                        if (pq_last) mma_commit(&bars->perq_done);
-                    }
-                    __syncwarp();
-                    ++g_mid; ++g_buf; ++rn;
-                    if (l == p.perq_layer) ++perq_count;
-                    if (++l_m == p.num_mid) { l_m = 0; it_m += 2; }
-                };
-                if (g_mid & 1) { try_mid(1, it_mid1, l_mid1, rnd1); try_mid(0, it_mid0, l_mid0, rnd0); }
-                else { try_mid(0, it_mid0, l_mid0, rnd0); try_mid(1, it_mid1, l_mid1, rnd1); }
             }
-        }
-    } else if (warp < 4 || (warp >= 9 && warp < 13)) {
-        // =============================================================== mid-layer epilogues (two chains)
-        const int c = (warp < 4) ? 0 : 1;                 // chain c owns tiles c, c+2, ...; act2 buffer c; A columns c
-        const int grp = warp & 3;                         // TMEM lane quarter this warp may access
-        const int pt = grp * 32 + lane;                   // point (row) of the tile handled by this thread
-        const uint32_t lane_base = (uint32_t)(grp * 32) << 16;
-        const uint32_t a_col = tmem + lane_base + kColA + (uint32_t)c * C::kACols;
-        uint32_t round = 0;
-        for (int it = c; it < ntiles; it += 2) {
-            const uint32_t ab = PRECISE ? 0u : (uint32_t)c;                              // activation buffer of this tile
-            const uint32_t au = PRECISE ? (uint32_t)it : ((uint32_t)it >> 1);           // its use count
-            // ---- mid layers
+            // ---- mid layers: 64 -> 64 (A stays in registers), the last one 64 -> 128 (into the big layer's B operand)
             int boff = 0;
-            for (int l = 0; l < p.num_mid; ++l, ++round) {
-                wait_bar(&bars->dmid_ready[c], round & 1, wsp ? wsp + WS_DMID_READY : nullptr);
-                tc_fence_after();
-                const int N = p.mid_N[l];
-                const bool last = (l == p.num_mid - 1);
-                if (last) {                         // every MMA that reads this chain's A columns has completed:
-                    tc_fence_before();              // the first-layer warps may write the next tile's operand
-                    mbar_arrive(&bars->a_free[c]);
-                }
-                const bool small = !PRECISE && (N == 64);
-                const uint32_t dcol = small ? kColDmidB : kColDmid;
-                for (int n0 = 0; n0 < N; n0 += 32) {
-                    uint32_t r[32];
-                    tmem_ld_x32(tmem + lane_base + dcol + n0, r);
-                    tmem_ld_wait();
-                    if (n0 + 32 >= N) {            // accumulator fully read: hand it to the other chain
-                        tc_fence_before();
-                        mbar_arrive(&bars->dmid_free[small ? 1 : 0]);
-                    }
-                    uint32_t v[16], vl[16];
+            for (int l = 0; l < p.num_mid; ++l) {
+                const float* bl = s_bias + boff;
+                const uint64_t w = dsc_mid[l], w_lo = dsc_mid_lo[l];
+                if (l < p.num_mid - 1) {
+                    float d[32];
 #pragma unroll
-                    for (int j4 = 0; j4 < 8; ++j4) {
-                        const float4 bb = *reinterpret_cast<const float4*>(s_bias + boff + n0 + 4 * j4);
-                        const float2 s01 = fadd2(make_float2(__uint_as_float(r[4 * j4]), __uint_as_float(r[4 * j4 + 1])), make_float2(bb.x, bb.y));
-                        const float2 s23 = fadd2(make_float2(__uint_as_float(r[4 * j4 + 2]), __uint_as_float(r[4 * j4 + 3])), make_float2(bb.z, bb.w));
-                        if (PRECISE) {
-                            pack_relu_split(s01.x, s01.y, v[2 * j4], vl[2 * j4]);
-                            pack_relu_split(s23.x, s23.y, v[2 * j4 + 1], vl[2 * j4 + 1]);
-                        } else {
-                            v[2 * j4] = pack_relu(s01.x, s01.y);
-                            v[2 * j4 + 1] = pack_relu(s23.x, s23.y);
-                        }
+                    for (int i = 0; i < 32; ++i) d[i] = 0.f;
+                    wgmma_fence();
+#pragma unroll
+                    for (int ks = 0; ks < 4; ++ks)
+                        mid_mma<PRECISE>(d, a[ks], reinterpret_cast<const uint32_t (&)[4]>(al[PRECISE ? ks : 0]), w + (uint64_t)(ks * 16), w_lo + (uint64_t)(ks * 16), ks > 0);
+                    wgmma_commit();
+                    wgmma_wait<0>();
+                    fence_regs(d);
+#pragma unroll
+                    for (int j = 0; j < 8; ++j) {
+                        const float2 bb = *reinterpret_cast<const float2*>(bl + 8 * j + 2 * q4);
+                        pack_act<PRECISE>(d[4 * j] + bb.x, d[4 * j + 1] + bb.y, a[j >> 1][(j & 1) * 2], al[j >> 1][PRECISE ? (j & 1) * 2 : 0]);
+                        pack_act<PRECISE>(d[4 * j + 2] + bb.x, d[4 * j + 3] + bb.y, a[j >> 1][(j & 1) * 2 + 1], al[j >> 1][PRECISE ? (j & 1) * 2 + 1 : 0]);
                     }
-                    if (!last) {
-                        // next layer's A operand (K index = channel, columns hold channel pairs); the MMA that read
-                        // this chain's A columns has completed (dmid_ready), so they can be overwritten in place
-                        uint32_t w[8];
+                } else {
+                    float d[64];
+#pragma unroll
+                    for (int i = 0; i < 64; ++i) d[i] = 0.f;
+                    wgmma_fence();
+#pragma unroll
+                    for (int ks = 0; ks < 4; ++ks)
+                        mid_mma<PRECISE>(d, a[ks], reinterpret_cast<const uint32_t (&)[4]>(al[PRECISE ? ks : 0]), w + (uint64_t)(ks * 16), w_lo + (uint64_t)(ks * 16), ks > 0);
+                    wgmma_commit();
+                    wgmma_wait<0>();
+                    fence_regs(d);
+                    wg_sync();                            // the previous tile's big-layer MMAs have read act2
+#pragma unroll
+                    for (int j = 0; j < 16; ++j) {
+                        const int k = 8 * j + 2 * q4;
+                        const float2 bb = *reinterpret_cast<const float2*>(bl + k);
 #pragma unroll
                         for (int h = 0; h < 2; ++h) {
-#pragma unroll
-                            for (int j = 0; j < 8; ++j) w[j] = v[h * 8 + j];
-                            tmem_st_x8(a_col + (uint32_t)(n0 / 2 + h * 8), w);
-                            if (PRECISE) {
-#pragma unroll
-                                for (int j = 0; j < 8; ++j) w[j] = vl[h * 8 + j];
-                                tmem_st_x8(a_col + 32u + (uint32_t)(n0 / 2 + h * 8), w);
-                            }
-                        }
-                    } else {
-                        // big layer's B operand [point row][channel K] K-major, LBO 128, SBO 2048
-                        uint8_t* dst = smem + kOffAct2 + ab * kAct2Bytes + (uint32_t)(pt >> 3) * 2048u + (uint32_t)(pt & 7) * 16u;
-#pragma unroll
-                        for (int j = 0; j < 4; ++j) {
-                            *reinterpret_cast<uint4*>(dst + (uint32_t)(n0 / 8 + j) * 128u) = make_uint4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
-                            if (PRECISE)   // lo image of the single activation buffer
-                                *reinterpret_cast<uint4*>(dst + kAct2Bytes + (uint32_t)(n0 / 8 + j) * 128u) = make_uint4(vl[4 * j], vl[4 * j + 1], vl[4 * j + 2], vl[4 * j + 3]);
+                            const int pt = r0 + 8 * h;
+                            const uint32_t off = (uint32_t)(pt >> 3) * 2048u + (uint32_t)j * 128u + (uint32_t)(pt & 7) * 16u + (uint32_t)q4 * 4u;
+                            uint32_t hi, lo = 0;
+                            pack_act<PRECISE>(d[4 * j + 2 * h] + bb.x, d[4 * j + 2 * h + 1] + bb.y, hi, lo);
+                            *reinterpret_cast<uint32_t*>(act2 + off) = hi;
+                            if (PRECISE) *reinterpret_cast<uint32_t*>(act2 + kAct2Bytes + off) = lo;
                         }
                     }
-                }
-                if (!last) {
-                    tmem_st_wait();
-                    if (l == p.num_mid - 2) wait_bar(&bars->act2_empty[ab], (au & 1) ^ 1, wsp ? wsp + WS_ACT2_EMPTY : nullptr);
-                    tc_fence_before();
-                    mbar_arrive(&bars->a_ready[c]);
-                } else {
                     fence_proxy_async_smem();
-                    tc_fence_before();
-                    mbar_arrive(&bars->act2_full[ab]);
+                    wg_sync();
                 }
-                boff += N;
+                boff += p.mid_N[l];
+            }
+            // ---- big layer 128 -> this CTA's channels: D[64 channels][64 points] per block, max over the points
+#pragma unroll
+            for (int c = 0; c < C::kChunks; ++c) {
+                float d0[32], d1[32];
+#pragma unroll
+                for (int i = 0; i < 32; ++i) { d0[i] = 0.f; d1[i] = 0.f; }
+                const uint64_t wa = dsc_w3 + (uint64_t)((uint32_t)c * (C::kChunkBytes >> 4)), wb = wa + (uint64_t)(16384u >> 4);
+                wgmma_fence();
+#pragma unroll
+                for (int ks = 0; ks < 8; ++ks) {
+                    const uint64_t x = dsc_act2 + (uint64_t)(ks * 16), o = (uint64_t)(ks * 16);
+                    if (PRECISE) {
+                        const uint64_t x_lo = x + (uint64_t)(kAct2Bytes >> 4), lo = (uint64_t)(32768u >> 4);
+                        wgmma_ss_n64(d0, wa + lo + o, x, ks > 0); wgmma_ss_n64(d0, wa + o, x_lo, 1); wgmma_ss_n64(d0, wa + o, x, 1);
+                        wgmma_ss_n64(d1, wb + lo + o, x, ks > 0); wgmma_ss_n64(d1, wb + o, x_lo, 1); wgmma_ss_n64(d1, wb + o, x, 1);
+                    } else {
+                        wgmma_ss_n64(d0, wa + o, x, ks > 0);
+                        wgmma_ss_n64(d1, wb + o, x, ks > 0);
+                    }
+                }
+                wgmma_commit();
+                wgmma_wait<0>();
+                fence_regs(d0);
+                fence_regs(d1);
+#pragma unroll
+                for (int j = 0; j < 8; ++j) {
+                    rmax[4 * c + 0] = fmaxf(rmax[4 * c + 0], fmaxf(d0[4 * j], d0[4 * j + 1]));
+                    rmax[4 * c + 1] = fmaxf(rmax[4 * c + 1], fmaxf(d0[4 * j + 2], d0[4 * j + 3]));
+                    rmax[4 * c + 2] = fmaxf(rmax[4 * c + 2], fmaxf(d1[4 * j], d1[4 * j + 1]));
+                    rmax[4 * c + 3] = fmaxf(rmax[4 * c + 3], fmaxf(d1[4 * j + 2], d1[4 * j + 3]));
+                }
             }
         }
-    } else if (warp >= 14) {
-        // =============================================================== first layer (fp32 FMA) for both chains
-        // thread = point = TMEM lane; produces the K = 64 fp16 A operand of the first mid layer of tile `it` in the
-        // A columns of chain it & 1 as soon as that chain has released them.
-        const int grp = warp & 3;
-        const int pt = grp * 32 + lane;
-        const int ct = tid - 14 * 32;
-        const uint32_t lane_base = (uint32_t)(grp * 32) << 16;
-        float* wq = s_wq;
-        const float* s_b0 = s_bias + 256;
-        int cur_q = -1;
-        // loads only: the centring subtraction happens at the use site one tile later, so the loads stay in flight
-        auto fetch = [&](int it2, float& x, float& y, float& z, float& cx, float& cy, float& cz) {
-            const int qi2 = it2 / tpq, tq2 = it2 - qi2 * tpq;
-            const size_t q2 = (size_t)stream + (size_t)qi2 * nstreams;
-            const int sgi = tq2 < p.seg[0].tiles ? 0 : 1;
-            const Seg& sg = p.seg[sgi];
-            int local = (tq2 - (sgi ? p.seg[0].tiles : 0)) * kTile + pt;
-            if (local >= sg.n) local = 0;                              // duplicate padding
-            const float* src = sg.ptr + (q2 * sg.n + local) * 3;
-            x = src[0]; y = src[1]; z = src[2];
-            cx = cy = cz = 0.f;
-            if (sg.center) { cx = p.query[q2 * 3 + 0]; cy = p.query[q2 * 3 + 1]; cz = p.query[q2 * 3 + 2]; }
-        };
-        float x = 0.f, y = 0.f, z = 0.f, pcx = 0.f, pcy = 0.f, pcz = 0.f;
-        if (ntiles > 0) fetch(0, x, y, z, pcx, pcy, pcz);
-        for (int it = 0; it < ntiles; ++it) {
-            const int c = it & 1;
-            const int qi = it / tpq;
-            if (qi != cur_q) {
-                // (W0 * R)^T for this query
-                const size_t q = (size_t)stream + (size_t)qi * nstreams;
-                asm volatile("bar.sync 3, 128;" ::: "memory");      // readers of the previous query's copy are done
-                if (ct < 64) {
-                    float w0 = p.W0[ct * 3 + 0], w1 = p.W0[ct * 3 + 1], w2 = p.W0[ct * 3 + 2];
-                    float r[9] = {1.f, 0.f, 0.f, 0.f, 1.f, 0.f, 0.f, 0.f, 1.f};
-                    if (p.R) {
+        // ---- the 4 lanes of a row hold disjoint point columns: combine, then one lane writes the channel
 #pragma unroll
-                        for (int i = 0; i < 9; ++i) r[i] = p.R[q * 9 + i];
-                    }
-                    wq[0 * 64 + ct] = w0 * r[0] + w1 * r[3] + w2 * r[6];
-                    wq[1 * 64 + ct] = w0 * r[1] + w1 * r[4] + w2 * r[7];
-                    wq[2 * 64 + ct] = w0 * r[2] + w1 * r[5] + w2 * r[8];
-                }
-                asm volatile("bar.sync 3, 128;" ::: "memory");
-                cur_q = qi;
-            }
-            x -= pcx; y -= pcy; z -= pcz;              // model.py:303
-            uint32_t v[32], vl[PRECISE ? 32 : 1];
-#pragma unroll
-            for (int j4 = 0; j4 < 16; ++j4) {
-                const float4 wx = *reinterpret_cast<const float4*>(wq + 0 * 64 + 4 * j4);
-                const float4 wy = *reinterpret_cast<const float4*>(wq + 1 * 64 + 4 * j4);
-                const float4 wz = *reinterpret_cast<const float4*>(wq + 2 * 64 + 4 * j4);
-                const float4 bb = *reinterpret_cast<const float4*>(s_b0 + 4 * j4);
-                // same association as the scalar form fma(wx, x, fma(wy, y, fma(wz, z, b))), two channels per FFMA2
-                const float2 xx = make_float2(x, x), yy = make_float2(y, y), zz = make_float2(z, z);
-                const float2 h01 = ffma2(make_float2(wx.x, wx.y), xx, ffma2(make_float2(wy.x, wy.y), yy, ffma2(make_float2(wz.x, wz.y), zz, make_float2(bb.x, bb.y))));
-                const float2 h23 = ffma2(make_float2(wx.z, wx.w), xx, ffma2(make_float2(wy.z, wy.w), yy, ffma2(make_float2(wz.z, wz.w), zz, make_float2(bb.z, bb.w))));
-                if (PRECISE) {
-                    pack_relu_split(h01.x, h01.y, v[2 * j4], vl[2 * j4]);
-                    pack_relu_split(h23.x, h23.y, v[2 * j4 + 1], vl[2 * j4 + 1]);
-                } else {
-                    v[2 * j4] = pack_relu(h01.x, h01.y);
-                    v[2 * j4 + 1] = pack_relu(h23.x, h23.y);
-                }
-            }
-            if (it + 1 < ntiles) fetch(it + 1, x, y, z, pcx, pcy, pcz);     // next tile's point, in flight during the store
-            wait_bar(&bars->a_free[c], (((uint32_t)it >> 1) & 1) ^ 1, wsp ? wsp + WS_A_FREE : nullptr);
-            tc_fence_after();
-            tmem_st_x32(tmem + lane_base + kColA + (uint32_t)c * C::kACols, v);
-            if (PRECISE) {
-                uint32_t (&vl32)[32] = reinterpret_cast<uint32_t (&)[32]>(vl);
-                tmem_st_x32(tmem + lane_base + kColA + (uint32_t)c * C::kACols + 32u, vl32);
-            }
-            tmem_st_wait();
-            // never trigger the last mid layer's MMA before this chain's act2 buffer is free: its epilogue must not
-            // hold the shared D_mid accumulator while waiting for the big layer
-            if (p.num_mid == 1) wait_bar(&bars->act2_empty[PRECISE ? 0 : c], ((PRECISE ? (uint32_t)it : ((uint32_t)it >> 1)) & 1) ^ 1, wsp ? wsp + WS_ACT2_EMPTY : nullptr);
-            tc_fence_before();
-            mbar_arrive(&bars->a_ready[c]);
+        for (int i = 0; i < 4 * C::kChunks; ++i) {
+            rmax[i] = fmaxf(rmax[i], __shfl_xor_sync(0xffffffffu, rmax[i], 1));
+            rmax[i] = fmaxf(rmax[i], __shfl_xor_sync(0xffffffffu, rmax[i], 2));
         }
-    } else {
-        // =============================================================== big-layer epilogue: max over the tile's points
-        const int ew = warp - 4;
-        const uint32_t lane_base = (uint32_t)(ew * 32) << 16;
-        const int ch_lane = ew * 32 + lane;
-        int it = 0;
-        for (int qi = 0; qi < nq; ++qi) {
-            const int q = stream + qi * nstreams;
-            float acc[C::kChunks];
+        if (q4 == 0) {
 #pragma unroll
-            for (int c = 0; c < C::kChunks; ++c) acc[c] = -INFINITY;
-            for (int tq = 0; tq < tpq; ++tq, ++it) {
-#pragma unroll
-                for (int c = 0; c < C::kChunks; ++c) {
-                    const uint32_t g = (uint32_t)(it * C::kChunks + c);
-                    const uint32_t stage = g & 1, use = g >> 1;
-                    wait_bar(&bars->d3_full[stage], use & 1, wsp ? wsp + WS_D3_FULL : nullptr);
-                    tc_fence_after();
-                    const uint32_t d = tmem + lane_base + kColD3 + stage * 128u;
-                    float m = acc[c];
-#pragma unroll
-                    for (int n0 = 0; n0 < 128; n0 += 64) {
-                        uint32_t r0[32], r1[32];
-                        tmem_ld_x32(d + n0, r0);
-                        tmem_ld_x32(d + n0 + 32, r1);
-                        tmem_ld_wait();
-                        if (n0 == 64) {             // accumulator fully read: release the stage before reducing
-                            tc_fence_before();
-                            mbar_arrive(&bars->d3_empty[stage]);
-                        }
-#pragma unroll
-                        for (int j = 0; j < 32; j += 2) m = fmax3(m, __uint_as_float(r0[j]), __uint_as_float(r0[j + 1]));
-#pragma unroll
-                        for (int j = 0; j < 32; j += 2) m = fmax3(m, __uint_as_float(r1[j]), __uint_as_float(r1[j + 1]));
-                    }
-                    acc[c] = m;
-                }
-            }
-#pragma unroll
-            for (int c = 0; c < C::kChunks; ++c) p.out[(size_t)q * 1024 + (part * C::kChunks + c) * 128 + ch_lane] = acc[c];
+            for (int i = 0; i < 4 * C::kChunks; ++i)
+                p.out[q * 1024 + (size_t)((part * C::kChunks + (i >> 2)) * 128 + ((i >> 1) & 1) * 64 + r0 + (i & 1) * 8)] = rmax[i];
         }
     }
-    if (STATS) ws_flush(p.wstats, warp == 8 ? 0 : (warp == 13 ? 1 : (warp < 4 ? 2 : (warp >= 14 ? 4 : (warp >= 9 ? 3 : 5)))), ws, t_begin);
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 8) tmem_dealloc(tmem, 512);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -684,7 +474,7 @@ struct TcWeights {
     const float* fold_bias[2] = {nullptr, nullptr};
     bool fc_on_tc = true;
     std::vector<void*> allocs;
-    int sm_count = 148;
+    int sm_count = 132;
     // profile of the dominant kernel (bench.py roofline)
     bool prof_on = false;
     std::vector<std::pair<cudaEvent_t, cudaEvent_t>> prof_events;
@@ -738,16 +528,9 @@ void launch_pass(Model& m, const TcStack& s, const Seg& s0, const Seg& s1, const
     p.perq_img = perq_img;
     p.w3_img = precise ? s.w3_img_p : s.w3_img;
     p.out = out;
-    p.wstats = nullptr;
+    for (int l = 0; l < s.num_mid; ++l)
+        P2S_CHECK(s.mid_N[l] == (l == s.num_mid - 1 ? 128 : 64), "pass kernel: mid layers must be 64 -> 64 ... -> 128");
     TcWeights& t = *m.tc;
-    static int wstats_on = -1;
-    if (wstats_on < 0) { const char* e = getenv("P2S_TC_WAITSTATS"); wstats_on = (e && e[0] == '1') ? 1 : 0; }
-    static long long* wstats_dev = nullptr;
-    if (wstats_on && !precise) {
-        if (!wstats_dev) P2S_CUDA(cudaMalloc(&wstats_dev, 6 * WS_SLOTS * sizeof(long long)));
-        P2S_CUDA(cudaMemsetAsync(wstats_dev, 0, 6 * WS_SLOTS * sizeof(long long), st));
-        p.wstats = wstats_dev;
-    }
     const int split = precise ? Cfg<true>::kSplit : Cfg<false>::kSplit;
     int streams = t.sm_count / split;
     if ((int64_t)streams > B) streams = (int)B;
@@ -759,27 +542,7 @@ void launch_pass(Model& m, const TcStack& s, const Seg& s0, const Seg& s1, const
         P2S_CUDA(cudaEventRecord(e0, st));
     }
     if (precise) P2S_LAUNCH(pointnet_pass_kernel<true>, grid, kThreads, Cfg<true>::kSmemBytes, st, p);
-    else if (wstats_on) {
-        static bool attr = false;
-        if (!attr) { P2S_CUDA(cudaFuncSetAttribute(pointnet_pass_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Cfg<false>::kSmemBytes)); attr = true; }
-        P2S_LAUNCH((pointnet_pass_kernel<false, true>), grid, kThreads, Cfg<false>::kSmemBytes, st, p);
-    } else P2S_LAUNCH(pointnet_pass_kernel<false>, grid, kThreads, Cfg<false>::kSmemBytes, st, p);
-    if (wstats_on && !precise) {
-        // diagnostics: average wait cycles per warp of each role, as a share of the role's lifetime
-        long long h[6 * WS_SLOTS];
-        P2S_CUDA(cudaMemcpyAsync(h, wstats_dev, sizeof(h), cudaMemcpyDeviceToHost, st));
-        P2S_CUDA(cudaStreamSynchronize(st));
-        static const char* roles[6] = {"big-issuer", "mid-issuer", "chain0", "chain1", "first-layer", "colmax"};
-        static const char* slots[WS_TOTAL] = {"act2_full", "d3_empty", "dmid_free", "dmid_ready", "act2_empty", "a_free", "d3_full"};
-        fprintf(stderr, "p2s waitstats: pass num_mid=%d perq=%d pts=%d+%d B=%lld precise=%d grid=%d\n", s.num_mid, perq_layer, s0.n, s1.n, (long long)B, (int)precise, grid);
-        for (int r = 0; r < 6; ++r) {
-            const double tot = (double)h[r * WS_SLOTS + WS_TOTAL];
-            if (tot <= 0) continue;
-            fprintf(stderr, "   %-12s", roles[r]);
-            for (int i = 0; i < WS_TOTAL; ++i) if (h[r * WS_SLOTS + i]) fprintf(stderr, " %s %.1f%%", slots[i], 100.0 * (double)h[r * WS_SLOTS + i] / tot);
-            fprintf(stderr, "  (role cycles per warp %.0f)\n", tot / (grid * (r == 0 || r == 1 ? 1.0 : 4.0)));
-        }
-    }
+    else P2S_LAUNCH(pointnet_pass_kernel<false>, grid, kThreads, Cfg<false>::kSmemBytes, st, p);
     if (prof) {
         P2S_CUDA(cudaEventRecord(e1, st));
         t.prof_events.emplace_back(e0, e1);

@@ -641,7 +641,7 @@ void sdf_to_volume(const int32_t* lin_idx, const float* sdf, int64_t Q, int res,
     const size_t smem_generic = (size_t)((X0 * Y0 * ZS + 15) & ~15) + (size_t)((X0 * Y0 * TZ + 15) & ~15) + (size_t)X0 * TY * TZ * 2;
     const size_t smem_fast = 4 * ((size_t)X0 * Y0 * (ZS / 4) + (size_t)TX * TY * 8 + (size_t)X0 * Y0 * 8 + (size_t)X0 * TY * 8);
     const size_t smem = pp.fast ? smem_fast : smem_generic;
-    int dev_id = 0, sms = 148, per_sm = 0;
+    int dev_id = 0, sms = 132, per_sm = 0;
     P2S_CUDA(cudaGetDevice(&dev_id));
     P2S_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev_id));
     const bool s5 = pp.fast && sigma == 5;

@@ -1,6 +1,6 @@
 """Drop-in for source/points_to_surf_eval.py: same CLI (parse_arguments), same entry point
 (points_to_surf_eval(eval_opt)), same output tree -- the per-query DataLoader + model loop
-(points_to_surf_eval.py:337-404) is replaced by the fused B200 pipeline (one C-ABI call per shape).
+(points_to_surf_eval.py:337-404) is replaced by the fused GPU pipeline (one C-ABI call per shape).
 
 Outputs per shape, as in the reference (points_to_surf_eval.py:199-294):
   <outdir>/{rec|eval}/eval/<name>.xyz.npy, .xyz.txt      signed distance per query

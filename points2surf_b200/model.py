@@ -1,6 +1,6 @@
 """Drop-in for source/points_to_surf_model.py: `PointsToSurfModel` with the reference's constructor
 signature (points_to_surf_model.py:238-240), parameter names and shapes (so the reference's checkpoints load,
-with or without the DataParallel 'module.' prefix), whose forward runs on the B200 kernels.
+with or without the DataParallel 'module.' prefix), whose forward runs on the CUDA kernels.
 
 Supported subset (SURVEY.md section 8b): sym_op='max', single_transformer=False, use_feat_stn=True,
 output_dim=2.  Anything else raises ValueError like the reference does for unknown options

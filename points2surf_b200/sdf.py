@@ -1,4 +1,4 @@
-"""Drop-in for the hot-path functions of source/sdf.py, on the B200 kernels."""
+"""Drop-in for the hot-path functions of source/sdf.py, on the CUDA kernels."""
 import os
 import time
 

@@ -1,4 +1,4 @@
-"""bench.py contract checks that need no GPU: the reference arm prints one JSON line with the agreed keys, the B200 arm
+"""bench.py contract checks that need no GPU: the reference arm prints one JSON line with the agreed keys, the GPU arm
 refuses to run without a CUDA device (no silent CPU fallback)."""
 import json
 import os

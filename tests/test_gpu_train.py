@@ -160,9 +160,8 @@ def test_train_iteration_matches_reference_digest(variant):
     # and (b) the full gradients of the CPU training oracle evaluated in float64 (the rounding-free truth).
     # Tolerances are relative L2: per tensor <= 1.5e-1, all gradients together <= 5e-2.  Any fp32 implementation sits a
     # few percent from the f64 truth here, because max-pool arg-max / ReLU decisions flip under rounding and the
-    # rotation gradient of the QSTN is a cancelling sum over 1300 points; measured on a B200 box with
-    # tools/train_noise_study.py (worst tensor / global): torch CPU autograd 0.009 / 0.006 (vanilla), 0.013 / 0.011
-    # (uniform); TrainStep over torch CUDA ops 0.021 / 0.011, 0.031 / 0.024; these kernels 0.033 / 0.023, 0.012 / 0.009.
+    # rotation gradient of the QSTN is a cancelling sum over 1300 points; tools/train_noise_study.py measures how far
+    # torch CPU autograd, TrainStep over torch CUDA ops and these kernels each sit from the float64 truth.
     v = synth.VARIANTS[variant]
     sd = synth.make_state_dict(variant, seed=TRAIN_SEEDS[variant])
     batch = train_fixture_batch(variant)

@@ -1,5 +1,5 @@
 """Measure the tensor-core path's logit error against the fp32 path on the benchmark workload and the number
-of sign-class mismatches that a guard band of a given width would leave (run on a B200):
+of sign-class mismatches that a guard band of a given width would leave (run on the GPU):
     python tools/guard_study.py [n_queries]
 """
 import os
