@@ -212,6 +212,20 @@ int p2s_nn_distance_dev(const float* a, int64_t na, const float* b, int64_t nb, 
 int p2s_chamfer_hausdorff_dev(const float* a, int64_t na, const float* b, int64_t nb, double* out4_host,
                               void* stream);
 
+/* ------------------------------------------------------------------ training targets ----------- */
+/* trimesh.proximity.signed_distance as called by sdf.get_signed_distance (source/sdf.py:318-348) for the query points
+ * of make_dataset.py:_get_and_save_query_pts (make_dataset.py:447-478).  Exhaustive and exact: the distance to the
+ * nearest triangle is the float64 minimum (an fp32 pass selects the faces to recompute within a stated error bound;
+ * ties -> lowest face index); zero-area faces count as segments / points.  Sign from the generalised winding number w
+ * (float64 solid angles of all faces): dist = +|d| if w > 0.5 or |d| <= 1e-8 (points on the surface are positive, like
+ * trimesh), else -|d|; inside is positive.  w equals trimesh's ray-parity inside test on closed, consistently oriented
+ * meshes; on meshes with holes or flipped faces the two can disagree.  A query with a non-finite coordinate gives NaN.
+ *   verts [V,3] fp32, faces [F,3] int32 (every index in [0, V), else an error; F > 0), query [Q,3] fp32
+ *   dist [Q] fp32; closest_face [Q] int32 or NULL; winding [Q] fp32 (w) or NULL.
+ * Bitwise deterministic, independent of how the queries are split across calls.  sync: index check read-back. */
+int p2s_mesh_signed_distance_dev(const float* verts, int64_t V, const int32_t* faces, int64_t F, const float* query,
+                                 int64_t Q, float* dist, int32_t* closest_face, float* winding, void* stream);
+
 /* ------------------------------------------------------------------ training-step primitives --- */
 /* Row a14 (SURVEY.md section 8a): loss + backward + SGD of source/points_to_surf_train.py:441-461,537-563 with the
  * train-mode BatchNorm of source/points_to_surf_model.py.  Activations are row-major [rows, C] fp32.  The host side

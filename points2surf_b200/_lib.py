@@ -74,6 +74,7 @@ SIGNATURES = {
     'p2s_op_axpy': (C.c_int, [_vp, _vp, _f32, _i64, _vp]),
     'p2s_op_sgd': (C.c_int, [_vp, _vp, _vp, _i64, _f32, _f32, _i32, _vp]),
     'p2s_chamfer_hausdorff_dev': (C.c_int, [_vp, _i64, _vp, _i64, C.POINTER(C.c_double), _vp]),
+    'p2s_mesh_signed_distance_dev': (C.c_int, [_vp, _i64, _vp, _i64, _vp, _i64, _vp, _vp, _vp, _vp]),
 }
 
 _lib = None

@@ -463,6 +463,14 @@ int p2s_chamfer_hausdorff_dev(const float* a, int64_t na, const float* b, int64_
     });
 }
 
+int p2s_mesh_signed_distance_dev(const float* verts, int64_t V, const int32_t* faces, int64_t F, const float* query,
+                                 int64_t Q, float* dist, int32_t* closest_face, float* winding, void* stream) {
+    return guarded([&] {
+        P2S_CHECK(verts && faces && ((query && dist) || Q == 0), "null argument");
+        mesh_signed_distance(verts, V, faces, F, query, Q, dist, closest_face, winding, as_stream(stream));
+    });
+}
+
 // ---- training-step primitives (train_ops.cu)
 #define P2S_OP(name, params, ...)                                   \
     int name params { return guarded([&] { __VA_ARGS__; }); }

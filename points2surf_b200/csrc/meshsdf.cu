@@ -1,0 +1,254 @@
+// K10: ground-truth signed distances from query points to a triangle mesh -- the training targets that
+// make_dataset.py:_get_and_save_query_pts writes to 05_query_dist (sdf.get_signed_distance, source/sdf.py:318-348, which
+// calls trimesh.proximity.signed_distance; trimesh is absent here).  Exhaustive and exact, no BVH:
+//   1. mesh_check_kernel: every face index in [0, V) (else an error, read back) and the largest |vertex coordinate|
+//      (the scale of the fp32 error bound below)
+//   2. meshsdf_slab_kernel: grid (query blocks, face slabs); every CTA stages tiles of its slab's triangles in shared
+//      memory, one query per thread, faces in ascending order.  Per face:
+//        - squared distance in fp32; every face whose fp32 value lies within kRelTol / the eps(scale) bound of the
+//          running fp32 minimum is recomputed in float64 and the float64 minimum kept (strict <: lowest face on ties).
+//          Degenerate and sliver faces (|n|^2 < 2^-10 * longest edge^4) skip the fp32 value and always go to float64.
+//        - float64 solid angle (Van Oosterom & Strackee 1983) summed into the slab's winding-number partial; zero-area
+//          faces contribute 0.
+//      -> per (slab, query): float64 d^2, face, float64 winding partial.  Slab boundaries depend on F only.
+//   3. meshsdf_finalize_kernel: slabs in ascending order (min d^2, strict <; winding sum) -> signed distance.
+// No float atomics anywhere: results are bitwise identical across runs and for any split of the query array.
+//
+// Sign: inside iff the generalised winding number w (Jacobson et al. 2013) > 0.5, inside is positive like trimesh;
+// |d| <= 1e-8 counts as on the surface and is positive (trimesh's tol.merge).  On a closed, consistently oriented mesh
+// w is 1 inside and 0 outside.  On a mesh with holes or inconsistent orientation w is fractional and can disagree with
+// trimesh's ray-parity test; the caller orients the mesh outward (points2surf_b200/sdf.py flips it when its signed
+// volume is negative, the global part of trimesh's fix_normals).
+#include "common.cuh"
+#include <cmath>
+
+namespace p2s {
+
+namespace {
+
+constexpr int kThreads = 128;      // queries per CTA
+constexpr int kTile = 128;         // faces per shared-memory tile (one staged per thread)
+constexpr int kMaxSlabs = 32;      // face slabs per query block
+constexpr int64_t kChunk = 1 << 18;   // queries per launch pair (bounds the per-slab partials to 20 B * 32 * 2^18)
+
+// fp32 error budget of the candidate test.  The fp32 squared distance of a well-shaped face (|n| >= 2^-5 * longest
+// edge^2, so that the fp32 normal is accurate to ~2^5 u) differs from the float64 one by far less than
+// 2^-10 * d^2 + 2 d eps + eps^2 with eps = 2^-12 * (|p|_inf + max |vertex coordinate|): the coordinate differences
+// carry u * scale, the normal direction 2^5 u, and the rest is a handful of roundings.  The face with the exact minimum
+// therefore always passes `d2f <= best32 + tol(best32)` (tol covers the error on both sides).
+constexpr float kRelTol = 1.0f / 1024.0f;
+constexpr float kEpsScale = 1.0f / 4096.0f;
+
+enum : unsigned char { kZeroArea = 1, kForce64 = 2 };
+
+// squared distance from p to the segment [a, b] (a point when a == b)
+template <class T>
+__device__ __forceinline__ T seg_dist2(T px, T py, T pz, T ax, T ay, T az, T bx, T by, T bz) {
+    const T ux = bx - ax, uy = by - ay, uz = bz - az;
+    const T wx = px - ax, wy = py - ay, wz = pz - az;
+    const T uu = ux * ux + uy * uy + uz * uz;
+    T t = uu > T(0) ? (ux * wx + uy * wy + uz * wz) / uu : T(0);
+    t = t < T(0) ? T(0) : (t > T(1) ? T(1) : t);
+    const T dx = wx - t * ux, dy = wy - t * uy, dz = wz - t * uz;
+    return dx * dx + dy * dy + dz * dz;
+}
+
+// squared distance from p to the triangle (a, b, c): the plane distance when p projects inside the triangle, else the
+// nearest edge.  A zero-area face is its three edges (a segment or a point).
+template <class T>
+__device__ __forceinline__ T tri_dist2(T px, T py, T pz, T ax, T ay, T az, T bx, T by, T bz, T cx, T cy, T cz,
+                                       bool zero_area) {
+    if (!zero_area) {
+        const T abx = bx - ax, aby = by - ay, abz = bz - az;
+        const T acx = cx - ax, acy = cy - ay, acz = cz - az;
+        const T nx = aby * acz - abz * acy, ny = abz * acx - abx * acz, nz = abx * acy - aby * acx;
+        const T nn = nx * nx + ny * ny + nz * nz;
+        const T apx = px - ax, apy = py - ay, apz = pz - az;
+        const T bpx = px - bx, bpy = py - by, bpz = pz - bz;
+        const T cpx = px - cx, cpy = py - cy, cpz = pz - cz;
+        const T bcx = cx - bx, bcy = cy - by, bcz = cz - bz;
+        const T cax = ax - cx, cay = ay - cy, caz = az - cz;
+        // p is on the inner side of edge (v, v') iff ((v' - v) x (p - v)) . n >= 0
+        const T e0 = (aby * apz - abz * apy) * nx + (abz * apx - abx * apz) * ny + (abx * apy - aby * apx) * nz;
+        const T e1 = (bcy * bpz - bcz * bpy) * nx + (bcz * bpx - bcx * bpz) * ny + (bcx * bpy - bcy * bpx) * nz;
+        const T e2 = (cay * cpz - caz * cpy) * nx + (caz * cpx - cax * cpz) * ny + (cax * cpy - cay * cpx) * nz;
+        if (nn > T(0) && e0 >= T(0) && e1 >= T(0) && e2 >= T(0)) {
+            const T h = nx * apx + ny * apy + nz * apz;
+            return h * h / nn;
+        }
+    }
+    T d = seg_dist2(px, py, pz, ax, ay, az, bx, by, bz);
+    d = fmin(d, seg_dist2(px, py, pz, bx, by, bz, cx, cy, cz));
+    return fmin(d, seg_dist2(px, py, pz, cx, cy, cz, ax, ay, az));
+}
+
+__global__ void __launch_bounds__(256)
+mesh_check_kernel(const float* __restrict__ verts, int64_t V, const int32_t* __restrict__ faces, int64_t F,
+                  unsigned* __restrict__ flags) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    bool bad = false;
+    unsigned m = 0;
+    if (i < 3 * F) {
+        const int32_t x = faces[i];
+        bad = x < 0 || x >= V;
+    }
+    if (i < 3 * V) m = __float_as_uint(fabsf(verts[i]));   // non-negative floats order like their bits; NaN sorts last
+    const unsigned nbad = __popc(__ballot_sync(0xffffffffu, bad));
+    m = __reduce_max_sync(0xffffffffu, m);
+    if ((threadIdx.x & 31) == 0) {
+        if (nbad) atomicAdd(flags, nbad);
+        atomicMax(flags + 1, m);
+    }
+}
+
+// grid (ceil(Q / kThreads), slabs): slab s covers faces [s * slab_len, min(F, (s + 1) * slab_len))
+__global__ void __launch_bounds__(kThreads)
+meshsdf_slab_kernel(const float* __restrict__ verts, const int32_t* __restrict__ faces, int64_t F, int64_t slab_len,
+                    const float* __restrict__ query, int64_t Q, float vmax, double* __restrict__ part_d2,
+                    int32_t* __restrict__ part_face, double* __restrict__ part_wind) {
+    __shared__ float sv[9][kTile];
+    __shared__ unsigned char sflag[kTile];
+    const int64_t i = (int64_t)blockIdx.x * kThreads + threadIdx.x;
+    float px = 0.f, py = 0.f, pz = 0.f;
+    if (i < Q) { px = query[3 * i]; py = query[3 * i + 1]; pz = query[3 * i + 2]; }
+    const double qx = px, qy = py, qz = pz;
+    const float eps = kEpsScale * (fmaxf(fabsf(px), fmaxf(fabsf(py), fabsf(pz))) + vmax);
+    float best32 = INFINITY, thr = INFINITY;
+    double best64 = INFINITY, wind = 0.0;
+    int32_t best_face = -1;
+    const int64_t f0 = (int64_t)blockIdx.y * slab_len, f1 = min(F, f0 + slab_len);
+    for (int64_t t = f0; t < f1; t += kTile) {
+        const int cnt = (int)min((int64_t)kTile, f1 - t);
+        __syncthreads();
+        if (threadIdx.x < cnt) {
+            const int64_t f = t + threadIdx.x;
+            float c[9];
+#pragma unroll
+            for (int k = 0; k < 3; ++k) {
+                const int64_t vi = faces[3 * f + k];
+                c[3 * k] = verts[3 * vi]; c[3 * k + 1] = verts[3 * vi + 1]; c[3 * k + 2] = verts[3 * vi + 2];
+            }
+#pragma unroll
+            for (int k = 0; k < 9; ++k) sv[k][threadIdx.x] = c[k];
+            // zero area: the float64 cross product of the edges is exactly 0 (no FMA contraction, so that the CPU
+            // restatement makes the same decision)
+            const double ux = (double)c[3] - c[0], uy = (double)c[4] - c[1], uz = (double)c[5] - c[2];
+            const double wx = (double)c[6] - c[0], wy = (double)c[7] - c[1], wz = (double)c[8] - c[2];
+            const double nx = __dsub_rn(__dmul_rn(uy, wz), __dmul_rn(uz, wy));
+            const double ny = __dsub_rn(__dmul_rn(uz, wx), __dmul_rn(ux, wz));
+            const double nz = __dsub_rn(__dmul_rn(ux, wy), __dmul_rn(uy, wx));
+            const double nn = nx * nx + ny * ny + nz * nz;
+            const double vx = (double)c[6] - c[3], vy = (double)c[7] - c[4], vz = (double)c[8] - c[5];
+            const double l2 = fmax(ux * ux + uy * uy + uz * uz, fmax(wx * wx + wy * wy + wz * wz, vx * vx + vy * vy + vz * vz));
+            const bool zero = nx == 0.0 && ny == 0.0 && nz == 0.0;
+            sflag[threadIdx.x] = zero ? (kZeroArea | kForce64) : (nn < (1.0 / 1024.0) * l2 * l2 ? kForce64 : 0);
+        }
+        __syncthreads();
+        if (i >= Q) continue;
+        for (int k = 0; k < cnt; ++k) {
+            const unsigned char fl = sflag[k];
+            const float ax = sv[0][k], ay = sv[1][k], az = sv[2][k];
+            const float bx = sv[3][k], by = sv[4][k], bz = sv[5][k];
+            const float cx = sv[6][k], cy = sv[7][k], cz = sv[8][k];
+            const bool zero = fl & kZeroArea;
+            float d2f = 0.f;
+            const bool force = fl & kForce64;
+            if (!force) d2f = tri_dist2<float>(px, py, pz, ax, ay, az, bx, by, bz, cx, cy, cz, false);
+            if (force || d2f <= thr) {
+                const double d2 = tri_dist2<double>(qx, qy, qz, ax, ay, az, bx, by, bz, cx, cy, cz, zero);
+                if (d2 < best64) { best64 = d2; best_face = (int32_t)(t + k); }
+                if (force) d2f = (float)d2;
+                if (d2f < best32) {
+                    best32 = d2f;
+                    thr = best32 + kRelTol * best32 + 2.f * sqrtf(best32) * eps + eps * eps;
+                }
+            }
+            if (!zero) {
+                const double Ax = ax - qx, Ay = ay - qy, Az = az - qz;
+                const double Bx = bx - qx, By = by - qy, Bz = bz - qz;
+                const double Cx = cx - qx, Cy = cy - qy, Cz = cz - qz;
+                const double la = sqrt(Ax * Ax + Ay * Ay + Az * Az);
+                const double lb = sqrt(Bx * Bx + By * By + Bz * Bz);
+                const double lc = sqrt(Cx * Cx + Cy * Cy + Cz * Cz);
+                const double det = Ax * (By * Cz - Bz * Cy) + Ay * (Bz * Cx - Bx * Cz) + Az * (Bx * Cy - By * Cx);
+                const double den = la * lb * lc + (Ax * Bx + Ay * By + Az * Bz) * lc + (Bx * Cx + By * Cy + Bz * Cz) * la +
+                                   (Cx * Ax + Cy * Ay + Cz * Az) * lb;
+                wind += atan2(det, den);   // half the solid angle of the face seen from q
+            }
+        }
+    }
+    if (i < Q) {
+        const int64_t o = (int64_t)blockIdx.y * Q + i;
+        part_d2[o] = best64;
+        part_face[o] = best_face;
+        part_wind[o] = wind;
+    }
+}
+
+__global__ void __launch_bounds__(256)
+meshsdf_finalize_kernel(const double* __restrict__ part_d2, const int32_t* __restrict__ part_face,
+                        const double* __restrict__ part_wind, int slabs, int64_t Q, float* __restrict__ dist,
+                        int32_t* __restrict__ closest_face, float* __restrict__ winding) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= Q) return;
+    double bd = INFINITY, w = 0.0;
+    int32_t bf = -1;
+    for (int s = 0; s < slabs; ++s) {
+        const double d = part_d2[(int64_t)s * Q + i];
+        if (d < bd) { bd = d; bf = part_face[(int64_t)s * Q + i]; }   // strict <: the lower slab (lower face) wins ties
+        w += part_wind[(int64_t)s * Q + i];
+    }
+    w *= 0.15915494309189533577;   // sum of half solid angles / (2 pi) = sum of solid angles / (4 pi)
+    const double d = sqrt(bd);
+    float out = (float)d;
+    if (bf < 0) out = NAN;                       // a non-finite query coordinate
+    else if (!(w > 0.5 || d <= 1e-8)) out = -out;
+    dist[i] = out;
+    if (closest_face) closest_face[i] = bf;
+    if (winding) winding[i] = (float)w;
+}
+
+struct Scratch {
+    DevBuf flags, d2, face, wind;
+};
+Scratch& scratch() {
+    static thread_local Scratch s;
+    return s;
+}
+
+}  // namespace
+
+void mesh_signed_distance(const float* verts, int64_t V, const int32_t* faces, int64_t F, const float* query, int64_t Q,
+                          float* dist, int32_t* closest_face, float* winding, cudaStream_t st) {
+    P2S_CHECK(V > 0 && F > 0, "empty mesh");
+    P2S_CHECK(V <= INT32_MAX && F <= INT32_MAX / 3, "mesh too large for int32 indices");
+    auto& sc = scratch();
+    unsigned* flags = sc.flags.as<unsigned>(2);   // [0] out-of-range face indices, [1] max |vertex coordinate| (bits)
+    P2S_CUDA(cudaMemsetAsync(flags, 0, 2 * sizeof(unsigned), st));
+    const int64_t n = 3 * std::max(V, F);
+    P2S_LAUNCH(mesh_check_kernel, (unsigned)cdiv(n, 256), 256, 0, st, verts, V, faces, F, flags);
+    unsigned h[2];
+    P2S_CUDA(cudaMemcpyAsync(h, flags, sizeof(h), cudaMemcpyDeviceToHost, st));
+    P2S_CUDA(cudaStreamSynchronize(st));
+    P2S_CHECK(h[0] == 0, "face index outside [0, V)");
+    float vmax;
+    memcpy(&vmax, &h[1], 4);
+    P2S_CHECK(std::isfinite(vmax), "non-finite vertex coordinate");
+    if (Q <= 0) return;
+    // slab boundaries are a function of F alone: the per-slab partials, and so the results, do not depend on Q
+    const int64_t slab_len = std::max<int64_t>(kTile, cdiv(cdiv(F, kMaxSlabs), kTile) * kTile);
+    const int slabs = (int)cdiv(F, slab_len);
+    const int64_t qc = std::min(Q, kChunk);
+    double* d2 = sc.d2.as<double>((size_t)slabs * qc);
+    int32_t* fc = sc.face.as<int32_t>((size_t)slabs * qc);
+    double* wn = sc.wind.as<double>((size_t)slabs * qc);
+    for (int64_t q0 = 0; q0 < Q; q0 += kChunk) {
+        const int64_t nq = std::min(kChunk, Q - q0);
+        P2S_LAUNCH(meshsdf_slab_kernel, dim3((unsigned)cdiv(nq, kThreads), (unsigned)slabs), kThreads, 0, st, verts, faces,
+                   F, slab_len, query + 3 * q0, nq, vmax, d2, fc, wn);
+        P2S_LAUNCH(meshsdf_finalize_kernel, (unsigned)cdiv(nq, 256), 256, 0, st, d2, fc, wn, slabs, nq, dist + q0,
+                   closest_face ? closest_face + q0 : nullptr, winding ? winding + q0 : nullptr);
+    }
+}
+
+}  // namespace p2s

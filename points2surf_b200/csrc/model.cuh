@@ -86,6 +86,9 @@ void mesh_sample(const float* verts, int64_t V, const int32_t* faces, int64_t F,
                  float* samples, int32_t* face_ids, cudaStream_t st);
 void nn_distance(const float* a, int64_t na, const float* b, int64_t nb, float* dist, int32_t* idx, cudaStream_t st);
 void chamfer_hausdorff(const float* a, int64_t na, const float* b, int64_t nb, double* out4_host, cudaStream_t st);
+// meshsdf.cu
+void mesh_signed_distance(const float* verts, int64_t V, const int32_t* faces, int64_t F, const float* query, int64_t Q,
+                          float* dist, int32_t* closest_face, float* winding, cudaStream_t st);
 // gemm_tn_tc.cu
 bool gemm_tn_tc_ok(const float* A, int lda, const float* B, int ldb, int64_t M, int N, int K);
 void launch_gemm_tn_tc(const float* A, int lda, const float* B, int ldb, float* C, int ldc, int64_t M, int N, int K,

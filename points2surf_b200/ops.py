@@ -276,6 +276,27 @@ def mesh_sample(verts, faces, num_samples, seed=0, return_face_ids=False):
     return (out, fid) if return_face_ids else out
 
 
+def mesh_signed_distance(verts, faces, query, return_face_ids=False, return_winding=False):
+    """Signed distance [Q] fp32 from every query point to the mesh, positive inside (the generalised winding number > 0.5)
+    and on the surface (|d| <= 1e-8) -- trimesh.proximity.signed_distance's convention (source/sdf.py:318-348).
+    Optionally also the closest face [Q] int32 (lowest index on ties) and the winding number [Q] fp32."""
+    verts = _dev(verts, torch.float32, 'verts')
+    faces = _dev(faces, torch.int32, 'faces')
+    q = _dev(query, torch.float32, 'query')
+    if verts.dim() != 2 or verts.shape[1] != 3 or faces.dim() != 2 or faces.shape[1] != 3 or q.dim() != 2 or q.shape[1] != 3:
+        raise P2SError('verts, faces and query must have shape [n, 3]')
+    Q = q.shape[0]
+    dist = torch.empty((Q,), dtype=torch.float32, device=q.device)
+    fid = torch.empty((Q,), dtype=torch.int32, device=q.device) if return_face_ids else None
+    wind = torch.empty((Q,), dtype=torch.float32, device=q.device) if return_winding else None
+    with torch.cuda.device(q.device):
+        check(_lib.load().p2s_mesh_signed_distance_dev(_ptr(verts), verts.shape[0], _ptr(faces), faces.shape[0], _ptr(q), Q,
+                                                       _ptr(dist), _ptr(fid) if fid is not None else None,
+                                                       _ptr(wind) if wind is not None else None, _stream()))
+    out = (dist,) + ((fid,) if return_face_ids else ()) + ((wind,) if return_winding else ())
+    return out if len(out) > 1 else dist
+
+
 def nn_distance(a, b):
     """Nearest neighbour in b of every point of a -> (dist [na] fp32, idx [na] int32)  (cKDTree.query(a, 1))."""
     a = _dev(a, torch.float32, 'a')

@@ -1,4 +1,5 @@
 """Drop-in for the hot-path functions of source/sdf.py, on the CUDA kernels."""
+import hashlib
 import os
 import time
 
@@ -96,6 +97,91 @@ def implicit_surface_to_mesh_directory(imp_surf_dist_ms_dir, query_pts_ms_dir, v
         v_out, m_out = os.path.join(vol_out_dir, f[:-8] + '.off'), os.path.join(mesh_out_dir, f[:-8] + '.ply')
         if _call_necessary([d_in, q_in], [v_out, m_out]):
             implicit_surface_to_mesh_file(d_in, q_in, v_out, m_out, grid_res, sigma, certainty_threshold)
+
+
+def _mesh_arrays(in_mesh):
+    """(vertices [V,3] float32, faces [F,3] int32) of an object with .vertices / .faces or of a (vertices, faces) pair."""
+    v, f = (in_mesh.vertices, in_mesh.faces) if hasattr(in_mesh, 'vertices') else in_mesh
+    v = np.ascontiguousarray(v, dtype=np.float32).reshape(-1, 3)
+    f = np.ascontiguousarray(f, dtype=np.int32).reshape(-1, 3)
+    if len(f) == 0 or f.min() < 0 or f.max() >= len(v):
+        raise ops.P2SError('mesh has no faces or a face index outside [0, V)')
+    return v, f
+
+
+def _orient_outward(verts, faces):
+    """The global part of trimesh's fix_normals (called at source/sdf.py:307): reverse every face when the mesh's signed
+    volume is negative.  Faces oriented inconsistently with their neighbours are not repaired."""
+    v = verts.astype(np.float64)
+    a, b, c = v[faces[:, 0]], v[faces[:, 1]], v[faces[:, 2]]
+    if np.einsum('ij,ij->', a, np.cross(b, c)) < 0.0:
+        return np.ascontiguousarray(faces[:, ::-1])
+    return faces
+
+
+def _query_pts_rng_draws(rng, num_query_pts, patch_radius, far_query_pts_ratio):
+    """What source/sdf.py:295,304-311 draws from the caller's stream, in its order: the close points' offsets along the
+    normal in [-patch_radius, patch_radius), then the far points in [-0.5, 0.5)^3.  -> (offsets [num_close], far [num_far,3])"""
+    num_far = int(num_query_pts * far_query_pts_ratio)
+    num_close = num_query_pts - num_far
+    offset = (rng.random(size=(num_close,)) - 0.5) * 2.0 * patch_radius
+    far = rng.random(size=(num_far, 3)) - 0.5
+    return offset, far
+
+
+def _sampler_seed(rng):
+    """Seed of the surface sampler, read from the caller's stream without drawing from it (so that the draws of
+    _query_pts_rng_draws stay the reference's): different streams and positions give different samples."""
+    _, key, pos = rng.get_state()[:3]
+    return int.from_bytes(hashlib.blake2b(key.tobytes() + int(pos).to_bytes(4, 'little'), digest_size=8).digest(), 'little')
+
+
+def _query_pts_and_faces(in_mesh, num_query_pts, patch_radius, far_query_pts_ratio, rng):
+    verts, faces = _mesh_arrays(in_mesh)
+    faces = _orient_outward(verts, faces)
+    seed = _sampler_seed(rng)
+    offset, far = _query_pts_rng_draws(rng, num_query_pts, patch_radius, far_query_pts_ratio)
+    dev = _device()
+    samples, face_id = ops.mesh_sample(torch.from_numpy(verts).to(dev), torch.from_numpy(faces).to(dev), len(offset), seed,
+                                       return_face_ids=True)
+    samples, face_id = samples.cpu().numpy().astype(np.float64), face_id.cpu().numpy()
+    v = verts.astype(np.float64)
+    f = faces[face_id]
+    n = np.cross(v[f[:, 1]] - v[f[:, 0]], v[f[:, 2]] - v[f[:, 0]])
+    n /= np.linalg.norm(n, axis=1, keepdims=True)                      # trimesh's unit face normals
+    n /= np.sqrt(np.linalg.norm(n, axis=1, keepdims=True))             # the reference's extra step (source/sdf.py:297-299)
+    close = samples + offset[:, None] * n
+    return np.concatenate((far, close), axis=0), face_id
+
+
+def get_query_pts_for_mesh(in_mesh, num_query_pts, patch_radius, far_query_pts_ratio=0.1, rng=None):
+    """source/sdf.py:288-315 -> float64 [num_query_pts, 3]: int(num_query_pts * far_query_pts_ratio) uniform points in
+    [-0.5, 0.5)^3, then points near the surface (area-weighted surface samples moved along their face normal by a uniform
+    offset in [-patch_radius, patch_radius)).  The offsets and the far points come from `rng` in the reference's order, so
+    the far half is bit-identical to the reference's for the same stream.  The surface samples come from the device
+    sampler (p2s_mesh_sample_dev, seeded from rng's state without drawing from it); the reference's are unseeded.
+    Of `in_mesh.fix_normals()` only the global flip is applied (faces reversed when the signed volume is negative), and
+    `in_mesh` is not modified.  `in_mesh`: anything with .vertices / .faces, or a (vertices, faces) pair."""
+    rng = np.random.RandomState() if rng is None else rng
+    return _query_pts_and_faces(in_mesh, num_query_pts, patch_radius, far_query_pts_ratio, rng)[0]
+
+
+def get_signed_distance(in_mesh, query_pts_ms, signed_distance_batch_size=1000):
+    """source/sdf.py:318-348 -> float64 [Q]: distance to the mesh, positive inside and on the surface (trimesh's
+    convention), on the device in one exhaustive pass (p2s_mesh_signed_distance_dev).  `signed_distance_batch_size` is
+    accepted and ignored: there is no memory blow-up to batch around.  The query points are rounded to float32 (what
+    05_query_pts stores).  The mesh is oriented outward like get_query_pts_for_mesh does (the sign comes from the
+    winding number, which depends on orientation; trimesh's ray test does not)."""
+    verts, faces = _mesh_arrays(in_mesh)
+    faces = _orient_outward(verts, faces)
+    dev = _device()
+    q = torch.from_numpy(np.ascontiguousarray(np.asarray(query_pts_ms).reshape(-1, 3), dtype=np.float32)).to(dev)
+    d = ops.mesh_signed_distance(torch.from_numpy(verts).to(dev), torch.from_numpy(faces).to(dev), q)
+    dists_ms = d.cpu().numpy().astype(np.float64)
+    num_nans, num_infs = int(np.isnan(dists_ms).sum()), int(np.isinf(dists_ms).sum())
+    if num_nans > 0 or num_infs > 0:
+        print('Error: Encountered {} NaN and {} Inf values in signed distance of {}.'.format(num_nans, num_infs, query_pts_ms))
+    return dists_ms
 
 
 def visualize_query_points(query_pts_ms, query_dist_ms, file_out_off):
