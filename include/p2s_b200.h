@@ -226,6 +226,35 @@ int p2s_chamfer_hausdorff_dev(const float* a, int64_t na, const float* b, int64_
 int p2s_mesh_signed_distance_dev(const float* verts, int64_t V, const int32_t* faces, int64_t F, const float* query,
                                  int64_t Q, float* dist, int32_t* closest_face, float* winding, void* stream);
 
+/* ------------------------------------------------------------------ input point clouds --------- */
+/* Simulated time-of-flight range scans: the BlenSor scans of make_dataset.py:sample_blensor (make_dataset.py:242-380,
+ * scanner settings blensor_script_template.py:80-96) merged in model space like _pcd_files_to_pts
+ * (make_dataset.py:147-239).  Scanner frame: the scanner sits at the origin and looks along +y; the image's wide axis
+ * (res_x columns, lens_angle_w) is z, its rows run along x.  Scan s places the model point p at R_s p + loc_s.  Pixel
+ * (row, col), row 0 at +x, col 0 at -z, casts the ray through the pixel centre (v, 1, u) / |(v, 1, u)| with
+ *   u = (2 (col + 1/2) / res_x - 1) tan(lens_angle_w / 2),  v = (1 - 2 (row + 1/2) / res_y) tan(lens_angle_h / 2).
+ * The ray hits the nearest surface at a distance t in (0, max_distance] (watertight ray-triangle test, no back-face
+ * culling, zero-area faces never hit, ties -> lowest face index).  The noisy range is t' = t + noise_mu + noise_sigma z
+ * with z standard normal from Philox4x32-10 keyed by (seed, first_scan + s, pixel).  Points are returned in model space,
+ * R_s^T (x - loc_s), compacted in (scan, row, col) order.
+ *   verts [V,3] fp32, faces [F,3] int32 (every index in [0, V), else an error; F > 0)
+ *   poses [S][12] float64 on the device: R_s row-major, then loc_s
+ *   pts_noisy [cap,3] fp32; pts_clean [cap,3] fp32 or NULL; face_ids [cap] int32 or NULL; hits_per_scan [S] int32 or NULL
+ *   total_host: the number of hits H.  Only the first min(H, cap) hits are written; H <= S * res_x * res_y.
+ * Bitwise deterministic and independent of how the scans are split across calls (with first_scan counting on).
+ * sync: count read-back. */
+typedef struct {
+    int32_t res_x, res_y;                        /* 176, 144 */
+    float lens_angle_w_deg, lens_angle_h_deg;    /* 43.6, 34.6: full field of view */
+    float max_distance;                          /* 10 */
+    float noise_mu, noise_sigma;                 /* Gaussian range noise */
+    int32_t first_scan;                          /* index of poses[0] in the shape's scan sequence (noise stream) */
+} p2s_scan_config;
+
+int p2s_range_scan_dev(const float* verts, int64_t V, const int32_t* faces, int64_t F, const double* poses, int64_t S,
+                       const p2s_scan_config* cfg, uint64_t seed, float* pts_noisy, float* pts_clean, int32_t* face_ids,
+                       int64_t cap, int32_t* hits_per_scan, int64_t* total_host, void* stream);
+
 /* ------------------------------------------------------------------ training-step primitives --- */
 /* Row a14 (SURVEY.md section 8a): loss + backward + SGD of source/points_to_surf_train.py:441-461,537-563 with the
  * train-mode BatchNorm of source/points_to_surf_model.py.  Activations are row-major [rows, C] fp32.  The host side

@@ -20,6 +20,11 @@ class ReconConfig(C.Structure):
                 ('seed', C.c_uint64), ('patch_radius', C.c_float), ('reserved', C.c_int32)]
 
 
+class ScanConfig(C.Structure):
+    _fields_ = [('res_x', C.c_int32), ('res_y', C.c_int32), ('lens_angle_w_deg', C.c_float), ('lens_angle_h_deg', C.c_float),
+                ('max_distance', C.c_float), ('noise_mu', C.c_float), ('noise_sigma', C.c_float), ('first_scan', C.c_int32)]
+
+
 PRECISION_FP32, PRECISION_TC = 0, 1
 SUBSAMPLE_WEIGHTED, SUBSAMPLE_UNIFORM = 0, 1
 
@@ -75,6 +80,8 @@ SIGNATURES = {
     'p2s_op_sgd': (C.c_int, [_vp, _vp, _vp, _i64, _f32, _f32, _i32, _vp]),
     'p2s_chamfer_hausdorff_dev': (C.c_int, [_vp, _i64, _vp, _i64, C.POINTER(C.c_double), _vp]),
     'p2s_mesh_signed_distance_dev': (C.c_int, [_vp, _i64, _vp, _i64, _vp, _i64, _vp, _vp, _vp, _vp]),
+    'p2s_range_scan_dev': (C.c_int, [_vp, _i64, _vp, _i64, _vp, _i64, C.POINTER(ScanConfig), C.c_uint64, _vp, _vp, _vp,
+                                     _i64, _vp, C.POINTER(_i64), _vp]),
 }
 
 _lib = None

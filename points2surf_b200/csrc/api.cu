@@ -471,6 +471,16 @@ int p2s_mesh_signed_distance_dev(const float* verts, int64_t V, const int32_t* f
     });
 }
 
+int p2s_range_scan_dev(const float* verts, int64_t V, const int32_t* faces, int64_t F, const double* poses, int64_t S,
+                       const p2s_scan_config* cfg, uint64_t seed, float* pts_noisy, float* pts_clean, int32_t* face_ids,
+                       int64_t cap, int32_t* hits_per_scan, int64_t* total_host, void* stream) {
+    return guarded([&] {
+        P2S_CHECK(verts && faces && cfg && total_host && (poses || S == 0), "null argument");
+        range_scan(verts, V, faces, F, poses, S, *cfg, seed, pts_noisy, pts_clean, face_ids, cap, hits_per_scan,
+                   total_host, as_stream(stream));
+    });
+}
+
 // ---- training-step primitives (train_ops.cu)
 #define P2S_OP(name, params, ...)                                   \
     int name params { return guarded([&] { __VA_ARGS__; }); }

@@ -297,6 +297,47 @@ def mesh_signed_distance(verts, faces, query, return_face_ids=False, return_wind
     return out if len(out) > 1 else dist
 
 
+SCANNER_DEFAULTS = dict(res_x=176, res_y=144, lens_angle_w=43.6, lens_angle_h=34.6, max_distance=10.0, noise_mu=0.0)
+
+
+def range_scan(verts, faces, rotations, locations, noise_sigma=0.0, seed=0, first_scan=0, **scanner):
+    """Simulated time-of-flight scans of a mesh (BlenSor's TOF scanner of make_dataset.py:sample_blensor, scanner frame
+    in include/p2s_b200.h).  rotations [S,3,3] and locations [S,3] place the model point p at R p + loc in front of the
+    scanner; scanner settings (`SCANNER_DEFAULTS`) can be overridden by keyword.  The range noise of scan s is keyed by
+    (seed, first_scan + s, pixel), so scanning the poses in pieces gives the same points.
+    -> (noisy [H,3] fp32, clean [H,3] fp32, face_ids [H] int32, hits_per_scan [S] int32), hits in (scan, row, col)
+    order, in model space."""
+    unknown = set(scanner) - set(SCANNER_DEFAULTS)
+    if unknown:
+        raise P2SError('unknown scanner settings: %s' % sorted(unknown))
+    s = dict(SCANNER_DEFAULTS, **scanner)
+    verts = _dev(verts, torch.float32, 'verts')
+    faces = _dev(faces, torch.int32, 'faces')
+    if verts.dim() != 2 or verts.shape[1] != 3 or faces.dim() != 2 or faces.shape[1] != 3:
+        raise P2SError('verts and faces must have shape [n, 3]')
+    dev = verts.device
+    rot = torch.as_tensor(rotations, dtype=torch.float64).to(dev).reshape(-1, 3, 3)
+    loc = torch.as_tensor(locations, dtype=torch.float64).to(dev).reshape(-1, 3)
+    if rot.shape[0] != loc.shape[0]:
+        raise P2SError('rotations and locations must describe the same number of scans')
+    S = rot.shape[0]
+    poses = torch.cat([rot.reshape(S, 9), loc], 1).contiguous()
+    cfg = _lib.ScanConfig(int(s['res_x']), int(s['res_y']), float(s['lens_angle_w']), float(s['lens_angle_h']),
+                          float(s['max_distance']), float(s['noise_mu']), float(noise_sigma), int(first_scan))
+    cap = S * int(s['res_x']) * int(s['res_y'])
+    noisy = torch.empty((cap, 3), dtype=torch.float32, device=dev)
+    clean = torch.empty((cap, 3), dtype=torch.float32, device=dev)
+    fid = torch.empty((cap,), dtype=torch.int32, device=dev)
+    hps = torch.empty((S,), dtype=torch.int32, device=dev)
+    total = C.c_int64(0)
+    with torch.cuda.device(dev):
+        check(_lib.load().p2s_range_scan_dev(_ptr(verts), verts.shape[0], _ptr(faces), faces.shape[0], _ptr(poses), S,
+                                             C.byref(cfg), int(seed) & (2 ** 64 - 1), _ptr(noisy), _ptr(clean), _ptr(fid),
+                                             cap, _ptr(hps), C.byref(total), _stream()))
+    H = total.value
+    return noisy[:H], clean[:H], fid[:H], hps
+
+
 def nn_distance(a, b):
     """Nearest neighbour in b of every point of a -> (dist [na] fp32, idx [na] int32)  (cKDTree.query(a, 1))."""
     a = _dev(a, torch.float32, 'a')
