@@ -259,7 +259,12 @@ int p2s_range_scan_dev(const float* verts, int64_t V, const int32_t* faces, int6
 /* Row a14 (SURVEY.md section 8a): loss + backward + SGD of source/points_to_surf_train.py:441-461,537-563 with the
  * train-mode BatchNorm of source/points_to_surf_model.py.  Activations are row-major [rows, C] fp32.  The host side
  * (points2surf_b200/train.py) sequences these like the reference's autograd graph.  All async on `stream`. */
-/* C[z][m][n] = act(sum_k A[z][m][k] W[z][n][k] + bias[n])   (torch conv1d(k=1) / linear / bmm forward) */
+/* Accuracy of both GEMMs, per output element, for operands anywhere in fp32's normal range:
+ *     |C - C_exact| <= gamma_K sum_k |a_k| |b_k| + 2^-40 K max_k |a_k| max_k |b_k|,   gamma_K = K 2^-24 / (1 - K 2^-24)
+ * (K = reduction length, the accumulate form counts the running value as one more term).  Large shapes run on the tensor
+ * cores in split precision after scaling every reduction vector by a power of two; the rest, and every shape under
+ * P2S_TRAIN_GEMM_FP32=1, on fp32 FMA.
+ * C[z][m][n] = act(sum_k A[z][m][k] W[z][n][k] + bias[n])   (torch conv1d(k=1) / linear / bmm forward) */
 int p2s_op_gemm_nt(const float* A, int64_t a_stride_z, int lda, const float* W, int64_t w_stride_z,
                    const float* bias, float* C, int64_t c_stride_z, int ldc, int M, int N, int K, int batch,
                    int relu, void* stream);

@@ -488,7 +488,8 @@ int p2s_range_scan_dev(const float* verts, int64_t V, const int32_t* faces, int6
 P2S_OP(p2s_op_gemm_nt, (const float* A, int64_t a_stride_z, int lda, const float* W, int64_t w_stride_z, const float* bias,
                         float* C, int64_t c_stride_z, int ldc, int M, int N, int K, int batch, int relu, void* stream),
        P2S_CHECK(A && W && C, "null argument");
-       // large unbatched shapes run on the tensor cores in split precision (fp32-level accuracy), the rest on fp32 FMA
+       // large unbatched shapes run on the tensor cores in split precision with power-of-two operand scaling, the rest on
+       // fp32 FMA; both meet the per-element bound stated in include/p2s_b200.h
        if (batch == 1 && gemm_nt_tc_ok(A, lda, C, ldc, M, N, K))
            launch_gemm_nt_tc(A, lda, W, bias, C, ldc, M, N, K, relu != 0, as_stream(stream));
        else

@@ -2,9 +2,11 @@
 // decoder 1024->512 (x2), 1024->256, 256->128; source/points_to_surf_model.py:62-64,120-122,335,343,348-350):
 //     C[M][N] = act( A[M][K] * W[N][K]^T + b ),  A fp32 row-major, W pre-packed operand images, fp32 accumulation
 //     in registers (wgmma), C fp32 row-major.
-// These layers produce the point rotation, the 64x64 feature transform and the logits, so they keep fp32-level
-// accuracy: every fp32 operand x is split into two fp16 numbers x_hi + x_lo (x_hi = fp16(x), x_lo = fp16(x - x_hi))
+// These layers produce the point rotation, the 64x64 feature transform and the logits, so they keep ~22-bit operands:
+// every fp32 operand x is split into two fp16 numbers x_hi + x_lo (x_hi = fp16(x), x_lo = fp16(x - x_hi))
 // and the product is evaluated as A_hi*W_hi + A_lo*W_hi + A_hi*W_lo (the dropped lo*lo term is ~2^-22 relative).
+// That holds while x_hi and x_lo are fp16 normal numbers (2^-3 <~ |x| <= 65504).  The training GEMMs (launch_gemm_nt_tc)
+// scale every row of A and W by a power of two first (split_exp, model.cuh); the inference chain's activations are O(1).
 // Three tensor-core passes cost nothing here: the FC tails are 1 % of the network's FLOPs.
 // One CTA per 128 x 128 output tile; K streamed in 32-wide stages (3-deep ring):
 //   warps 0-3   producers (fp32 A only): thread = output row; load 32 fp32 of that row, split, store the two K-major
@@ -45,11 +47,15 @@ __device__ __forceinline__ void split_half2(float x0, float x1, uint32_t& hi, ui
 // ([M/128][K/32][hi | lo][128 x 32 fp16], the W layout): then the producers have nothing to do and both operands of a k-step
 // arrive by bulk copy (every A element is loaded and split once instead of once per N tile).
 // pack_img == 3 writes C as the NEXT layer's operand image (k-steps out_kt_off.. of out_kt_total).
+// kScaled (training GEMMs only): rows of A and W scaled by 2^a_exp[m] / 2^w_exp[n] (model.cuh, split_exp); a template
+// parameter so that the inference instantiation carries none of it.
+template <bool kScaled>
 __global__ void __launch_bounds__(kFcThreads, 1) fc_tc_kernel(const float* __restrict__ A, int lda, const uint8_t* __restrict__ Wimg,
                                                               const float* __restrict__ bias, float* __restrict__ C, int ldc,
                                                               int M, int N, int K, int relu, int pack_img,
                                                               const float* __restrict__ in_bias, int in_relu,
-                                                              const uint8_t* __restrict__ Aimg, int out_kt_total, int out_kt_off) {
+                                                              const uint8_t* __restrict__ Aimg, int out_kt_total, int out_kt_off,
+                                                              const int* __restrict__ a_exp, const int* __restrict__ w_exp) {
     extern __shared__ __align__(1024) uint8_t smem[];
     FcBars* bars = reinterpret_cast<FcBars*>(smem + kStages * (kStageA + kStageB));
     const int tid = threadIdx.x, warp = tid >> 5;
@@ -69,6 +75,10 @@ __global__ void __launch_bounds__(kFcThreads, 1) fc_tc_kernel(const float* __res
         // register double buffer: the loads of k-step kt + 1 are in flight while k-step kt is converted and stored
         float4 v[8], nv[8];
         const bool row_ok = row < M;
+        // training GEMMs (a_exp set, no in_bias): the row is scaled by 2^s before the split (model.cuh, split_exp)
+        const int sa_row = kScaled && row_ok ? a_exp[row] : 0;
+        const bool fa_one = sa_row >= -126 && sa_row <= 127;            // 2^s is a normal float: one multiplication
+        const float2 fa = fa_one ? make_float2(__int_as_float((127 + sa_row) << 23), 1.f) : split_factors(sa_row);
 #pragma unroll
         for (int j = 0; j < 8; ++j) v[j] = row_ok ? *reinterpret_cast<const float4*>(src + j * 4) : make_float4(0.f, 0.f, 0.f, 0.f);
         for (int kt = 0; kt < nk; ++kt) {
@@ -88,6 +98,15 @@ __global__ void __launch_bounds__(kFcThreads, 1) fc_tc_kernel(const float* __res
                     if (in_relu) {
 #pragma unroll
                         for (int e = 0; e < 8; ++e) x[e] = fmaxf(x[e], 0.f);
+                    }
+                }
+                if (kScaled) {
+                    if (fa_one) {
+#pragma unroll
+                        for (int e = 0; e < 8; ++e) x[e] *= fa.x;
+                    } else {
+#pragma unroll
+                        for (int e = 0; e < 8; ++e) x[e] = x[e] * fa.x * fa.y;
                     }
                 }
                 uint32_t hi[4], lo[4];
@@ -144,14 +163,23 @@ __global__ void __launch_bounds__(kFcThreads, 1) fc_tc_kernel(const float* __res
         // ---- epilogue: thread holds rows r, r + 8 and column pairs 8 j + 2 (t % 4) of the tile
         const int q = t & 3;
         const float* b = bias + nt * 128;
+        int2 sw[16];                                         // column scales of the training GEMMs, loaded up front
+#pragma unroll
+        for (int j = 0; j < 16; ++j) sw[j] = kScaled && nt * 128 + 8 * j + 2 * q < N ? __ldg(reinterpret_cast<const int2*>(w_exp + nt * 128 + 8 * j + 2 * q)) : make_int2(0, 0);
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
             const int r = wg * 64 + (t >> 5) * 16 + ((t & 31) >> 2) + h * 8, row = m0 + r;
+            const int sa = kScaled && row < M ? a_exp[row] : 0;
 #pragma unroll
             for (int j = 0; j < 16; ++j) {
                 const int col = 8 * j + 2 * q;
                 if (pack_img != 3 && (row >= M || nt * 128 + col >= N)) continue;   // padded rows / N tile (N % 4 == 0)
-                float x0 = acc[4 * j + 2 * h] + b[col], x1 = acc[4 * j + 2 * h + 1] + b[col + 1];
+                float a0 = acc[4 * j + 2 * h], a1 = acc[4 * j + 2 * h + 1];
+                if (kScaled) {       // undo the operand scales: exact unless the product leaves fp32's range
+                    a0 = split_unscale(a0, -(sa + sw[j].x));
+                    a1 = split_unscale(a1, -(sa + sw[j].y));
+                }
+                float x0 = a0 + b[col], x1 = a1 + b[col + 1];
                 if (relu) { x0 = fmaxf(x0, 0.f); x1 = fmaxf(x1, 0.f); }
                 if (pack_img == 3) {
                     // C as the next layer's A operand image: 32 columns are exactly one k-step of that layer
@@ -220,14 +248,16 @@ __global__ void __launch_bounds__(256) pack_a_kernel(const float* __restrict__ A
     }
 }
 
-// same image for N rows padded with zeros to Npad (multiple of 128)
-__global__ void pack_fc_pad_kernel(const float* __restrict__ W, int N, int Npad, int K, uint8_t* __restrict__ img) {
+// same image for N rows padded with zeros to Npad (multiple of 128), row n scaled by 2^w_exp[n] (model.cuh, split_exp)
+__global__ void pack_fc_pad_kernel(const float* __restrict__ W, int N, int Npad, int K, const int* __restrict__ w_exp,
+                                   uint8_t* __restrict__ img) {
     int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (e >= (int64_t)Npad * K) return;
     int n = (int)(e / K), k = (int)(e % K);
     int nt = n >> 7, r = n & 127, kt = k / kBK, kk = k % kBK;
     size_t off = ((size_t)nt * (K / kBK) + kt) * kStageB + (size_t)(r >> 3) * 512 + (size_t)(kk >> 3) * 128 + (size_t)(r & 7) * 16 + (size_t)(kk & 7) * 2;
-    const float w = n < N ? W[e] : 0.f;
+    const float2 f = split_factors(n < N ? w_exp[n] : 0);
+    const float w = n < N ? W[e] * f.x * f.y : 0.f;
     const __half h = __float2half_rn(w);
     *reinterpret_cast<__half*>(img + off) = h;
     *reinterpret_cast<__half*>(img + off + kHalf) = __float2half_rn(w - __half2float(h));
@@ -249,20 +279,27 @@ uint8_t* fc_tc_pack(const Layer& L, std::vector<void*>& allocs) {
 void fc_tc_init() {
     static bool done = false;
     if (!done) {
-        P2S_CUDA(cudaFuncSetAttribute(fc_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFcSmem));
+        P2S_CUDA(cudaFuncSetAttribute(fc_tc_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFcSmem));
+        P2S_CUDA(cudaFuncSetAttribute(fc_tc_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFcSmem));
         done = true;
     }
 }
 
 void launch_fc_tc(const float* A, int lda, const uint8_t* Wimg, const float* bias, float* C, int ldc,
-                  int64_t M, int N, int K, bool relu, cudaStream_t st, int pack_img, const float* in_bias, bool in_relu) {
+                  int64_t M, int N, int K, bool relu, cudaStream_t st, int pack_img, const float* in_bias, bool in_relu,
+                  const int* a_exp, const int* w_exp) {
     if (M <= 0) return;
+    P2S_CHECK(!(a_exp || w_exp) || (a_exp && w_exp && !pack_img && !in_bias), "operand scales need both exponents and a plain fp32 C");
     const bool padded_ok = !pack_img && N % 4 == 0 && N >= 64 && K % kBK == 0;   // partial last N tile (training GEMMs)
     P2S_CHECK((fc_tc_supported(N, K) || padded_ok) && lda % 4 == 0 && (pack_img ? N == 4096 : ldc % 4 == 0), "bad FC shape for the tensor-core kernel");
     P2S_CHECK(cdiv(M, 128) <= 65535, "too many rows for one launch");
     dim3 grid((unsigned)cdiv(N, 128), (unsigned)cdiv(M, 128), 1);
-    P2S_LAUNCH(fc_tc_kernel, grid, kFcThreads, kFcSmem, st, A, lda, Wimg, bias, C, ldc, (int)M, N, K, relu ? 1 : 0, pack_img, in_bias, in_relu ? 1 : 0,
-               (const uint8_t*)nullptr, 0, 0);
+    if (a_exp)
+        P2S_LAUNCH(fc_tc_kernel<true>, grid, kFcThreads, kFcSmem, st, A, lda, Wimg, bias, C, ldc, (int)M, N, K, relu ? 1 : 0, pack_img, in_bias,
+                   in_relu ? 1 : 0, (const uint8_t*)nullptr, 0, 0, a_exp, w_exp);
+    else
+        P2S_LAUNCH(fc_tc_kernel<false>, grid, kFcThreads, kFcSmem, st, A, lda, Wimg, bias, C, ldc, (int)M, N, K, relu ? 1 : 0, pack_img, in_bias,
+                   in_relu ? 1 : 0, (const uint8_t*)nullptr, 0, 0, (const int*)nullptr, (const int*)nullptr);
 }
 
 size_t fc_tc_a_image_bytes(int64_t M, int K) { return (size_t)cdiv(M, 128) * (size_t)(K / kBK) * kStageA; }
@@ -283,8 +320,8 @@ void launch_fc_tc_img(const uint8_t* Aimg, const uint8_t* Wimg, const float* bia
               "bad FC shape for the tensor-core kernel (operand-image mode)");
     P2S_CHECK(cdiv(M, 128) <= 65535, "too many rows for one launch");
     dim3 grid((unsigned)(N / 128), (unsigned)cdiv(M, 128), 1);
-    P2S_LAUNCH(fc_tc_kernel, grid, kFcThreads, kFcSmem, st, (const float*)nullptr, 0, Wimg, bias, reinterpret_cast<float*>(C), ldc, (int)M, N, K, relu ? 1 : 0,
-               out_mode, (const float*)nullptr, 0, Aimg, out_kt_total, out_kt_off);
+    P2S_LAUNCH(fc_tc_kernel<false>, grid, kFcThreads, kFcSmem, st, (const float*)nullptr, 0, Wimg, bias, reinterpret_cast<float*>(C), ldc, (int)M, N, K, relu ? 1 : 0,
+               out_mode, (const float*)nullptr, 0, Aimg, out_kt_total, out_kt_off, (const int*)nullptr, (const int*)nullptr);
 }
 
 // images of a raw fp32 matrix W[N][K] (device pointer)
@@ -297,8 +334,74 @@ uint8_t* fc_tc_pack_raw(const float* W, int N, int K, std::vector<void*>& allocs
     return (uint8_t*)p;
 }
 
-// Split-precision tensor-core GEMM for weights that change between calls (training): packs W [N][K] into a reusable
-// scratch image on `st`, then runs fc_tc_kernel.  Stream order makes the scratch reuse safe.  bias may be null.
+namespace {
+
+// split_exp(max |x|) per row: one warp per row (W may sit at any float offset of the flat parameter buffer: scalar loads)
+__global__ void __launch_bounds__(256) split_exp_rows_kernel(const float* __restrict__ X, int ld, int64_t rows, int cols,
+                                                             int* __restrict__ out) {
+    const int64_t r = (int64_t)blockIdx.x * 8 + (threadIdx.x >> 5);
+    if (r >= rows) return;
+    const float* x = X + r * ld;
+    float m = 0.f;
+    for (int c = threadIdx.x & 31; c < cols; c += 32) m = fmaxf(m, fabsf(x[c]));
+#pragma unroll
+    for (int o = 16; o; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+    if ((threadIdx.x & 31) == 0) out[r] = split_exp(m);
+}
+
+// max |x| per column: a CTA covers 128 columns (32 lanes x float4) of a slice of rows; per-CTA maxima are merged with
+// atomicMax on the float bits (order-preserving for non-negative floats)
+__global__ void __launch_bounds__(256) absmax_cols_kernel(const float* __restrict__ X, int ld, int64_t rows, int cols,
+                                                          unsigned* __restrict__ out) {
+    __shared__ float4 red[8][32];
+    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+    const int c = blockIdx.x * 128 + lane * 4;
+    float4 m = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (c < cols) {
+        for (int64_t r = (int64_t)blockIdx.y * 8 + w; r < rows; r += (int64_t)gridDim.y * 8) {
+            const float4 v = *reinterpret_cast<const float4*>(X + r * ld + c);
+            m.x = fmaxf(m.x, fabsf(v.x)); m.y = fmaxf(m.y, fabsf(v.y)); m.z = fmaxf(m.z, fabsf(v.z)); m.w = fmaxf(m.w, fabsf(v.w));
+        }
+    }
+    red[w][lane] = m;
+    __syncthreads();
+    if (w == 0 && c < cols) {
+#pragma unroll
+        for (int i = 1; i < 8; ++i) {
+            const float4 o = red[i][lane];
+            m.x = fmaxf(m.x, o.x); m.y = fmaxf(m.y, o.y); m.z = fmaxf(m.z, o.z); m.w = fmaxf(m.w, o.w);
+        }
+        atomicMax(out + c, __float_as_uint(m.x));
+        atomicMax(out + c + 1, __float_as_uint(m.y));
+        atomicMax(out + c + 2, __float_as_uint(m.z));
+        atomicMax(out + c + 3, __float_as_uint(m.w));
+    }
+}
+
+}  // namespace
+
+void launch_split_exp_rows(const float* X, int ld, int64_t rows, int cols, int* out, cudaStream_t st) {
+    if (rows <= 0) return;
+    P2S_LAUNCH(split_exp_rows_kernel, (unsigned)cdiv(rows, 8), 256, 0, st, X, ld, rows, cols, out);
+}
+
+void launch_absmax_cols(const float* X, int ld, int64_t rows, int cols, unsigned* out, cudaStream_t st) {
+    P2S_CHECK(cols % 4 == 0 && ld % 4 == 0 && (uintptr_t)X % 16 == 0, "absmax_cols: unaligned rows");
+    P2S_CUDA(cudaMemsetAsync(out, 0, sizeof(unsigned) * (size_t)cols, st));
+    if (rows <= 0) return;
+    int dev = 0, sms = 132;
+    P2S_CUDA(cudaGetDevice(&dev));
+    P2S_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+    const int64_t cb = cdiv(cols, 128);
+    const int64_t slices = std::min<int64_t>(cdiv(rows, 64), std::max<int64_t>(1, cdiv(8 * (int64_t)sms, cb)));
+    P2S_LAUNCH(absmax_cols_kernel, dim3((unsigned)cb, (unsigned)std::min<int64_t>(slices, 65535)), 256, 0, st, X, ld, rows, cols, out);
+}
+
+// Split-precision tensor-core GEMM for weights that change between calls (training): takes the row scales of A and W,
+// packs the scaled W [N][K] into a reusable scratch image on `st`, then runs fc_tc_kernel with the scaled A rows (see
+// split_exp in model.cuh).  Stream order makes the scratch reuse safe.  bias may be null.
+// Every output element meets |C - C_exact| <= gamma_K sum_k |a_k b_k| + 2^-40 K max_k |a_k| max_k |b_k| (up to the
+// tensor cores' accumulation order) at any operand scale inside fp32's normal range.
 bool gemm_nt_tc_ok(const float* A, int lda, const float* C, int ldc, int64_t M, int N, int K) {
     static int disabled = -1;
     if (disabled < 0) {
@@ -311,11 +414,13 @@ bool gemm_nt_tc_ok(const float* A, int lda, const float* C, int ldc, int64_t M, 
 
 void launch_gemm_nt_tc(const float* A, int lda, const float* W, const float* bias, float* C, int ldc, int64_t M, int N,
                        int K, bool relu, cudaStream_t st) {
-    static thread_local DevBuf img, zeros;
+    static thread_local DevBuf img, zeros, amax;
     static thread_local bool zeroed = false;
     fc_tc_init();
     const int Npad = (int)(cdiv(N, 128) * 128);
     uint8_t* wimg = reinterpret_cast<uint8_t*>(img.get((size_t)Npad * K * 4));
+    int* a_exp = amax.as<int>((size_t)M + N + 2);
+    int* w_exp = a_exp + ((M + 1) & ~(int64_t)1);          // 8-byte aligned: the epilogue reads column pairs
     if (!bias) {
         float* z = zeros.as<float>(4096);
         if (!zeroed) {
@@ -324,8 +429,10 @@ void launch_gemm_nt_tc(const float* A, int lda, const float* W, const float* bia
         }
         bias = z;
     }
-    P2S_LAUNCH(pack_fc_pad_kernel, (unsigned)cdiv((int64_t)Npad * K, 256), 256, 0, st, W, N, Npad, K, wimg);
-    launch_fc_tc(A, lda, wimg, bias, C, ldc, M, N, K, relu, st, 0);
+    launch_split_exp_rows(A, lda, M, K, a_exp, st);
+    launch_split_exp_rows(W, K, N, K, w_exp, st);
+    P2S_LAUNCH(pack_fc_pad_kernel, (unsigned)cdiv((int64_t)Npad * K, 256), 256, 0, st, W, N, Npad, K, w_exp, wimg);
+    launch_fc_tc(A, lda, wimg, bias, C, ldc, M, N, K, relu, st, 0, nullptr, false, a_exp, w_exp);
 }
 
 }  // namespace p2s

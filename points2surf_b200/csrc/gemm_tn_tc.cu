@@ -3,8 +3,11 @@
 // The contraction runs over the rows m (up to 1.3 M of them), so both operands are "transposed" with respect to the
 // K-major layout wgmma wants.  The producers do the transposition on the fly: a warp reads whole rows (coalesced),
 // every thread ends up with an 8 (m) x 4 (n) block and writes four 16-byte core-matrix rows of the K-major operand
-// image (k = m), split into fp16 hi / lo parts; three MMAs per k-step (lo*hi + hi*lo + hi*hi) keep fp32-level accuracy
-// (same scheme as fc_tc.cu).  One CTA = one 128 (n) x 128 (k) output tile x one slice of the rows; partial tiles are
+// image (k = m), split into fp16 hi / lo parts; three MMAs per k-step (lo*hi + hi*lo + hi*hi).  Every column of both
+// operands is first scaled by a power of two chosen from its maximum over all M rows (absmax_cols_kernel, split_exp in
+// model.cuh), so the split keeps ~22 bits at any operand scale, and the epilogue undoes the scales.  Per element,
+// |C - C_exact| <= gamma_M sum_m |a_m b_m| + 2^-40 M max_m |a_m| max_m |b_m| (up to the tensor cores' accumulation order),
+// the same bound as fp32 FMA accumulation plus a floor for parts ~2^-40 below a column's maximum.  One CTA = one 128 (n) x 128 (k) output tile x one slice of the rows; partial tiles are
 // added to C with fp32 atomics (C is zeroed or holds the running gradient).
 //   warps 0-3   A-operand producers (dZ tile 32 rows x 128 n)
 //   warps 4-7   B-operand producers (X tile 32 rows x 128 k)
@@ -30,10 +33,10 @@ struct Bars {
     uint64_t full[kStages], empty[kStages];
 };
 
-// Fill one operand image (hi | lo) from src[m][c0 .. c0+127] (row stride ld), rows m0 .. m0+31 (< m_end), cols < ncols.
-// t = thread index within the 128 producers of this operand.
+// Fill one operand image (hi | lo) from src[m][c0 .. c0+127] (row stride ld), rows m0 .. m0+31 (< m_end), cols < ncols,
+// column c0 + (t % 32) * 4 + i scaled by fs[i].x * fs[i].y.  t = thread index within the 128 producers of this operand.
 __device__ __forceinline__ void fill_operand(uint8_t* dst, const float* __restrict__ src, int ld, int64_t m0, int64_t m_end,
-                                             int c0, int ncols, int t) {
+                                             int c0, int ncols, int t, const float2 (&fs)[4]) {
     const int col = c0 + (t & 31) * 4;        // 4 consecutive n (or k)
     const int rg = t >> 5;                    // row group: rows rg*8 .. rg*8+7  == k-chunk rg of the operand
     float4 v[8];
@@ -48,7 +51,7 @@ __device__ __forceinline__ void fill_operand(uint8_t* dst, const float* __restri
         const int i = (ii + (lane >> 1)) & 3;                       // rotate to spread the shared-memory banks
         float x[8];
 #pragma unroll
-        for (int j = 0; j < 8; ++j) x[j] = i == 0 ? v[j].x : (i == 1 ? v[j].y : (i == 2 ? v[j].z : v[j].w));
+        for (int j = 0; j < 8; ++j) x[j] = (i == 0 ? v[j].x : (i == 1 ? v[j].y : (i == 2 ? v[j].z : v[j].w))) * fs[i].x * fs[i].y;
         uint32_t hi[4], lo[4];
 #pragma unroll
         for (int e = 0; e < 4; ++e) {
@@ -67,7 +70,8 @@ __device__ __forceinline__ void fill_operand(uint8_t* dst, const float* __restri
 
 __global__ void __launch_bounds__(512, 1)
 gemm_tn_tc_kernel(const float* __restrict__ A, int lda, const float* __restrict__ B, int ldb, float* __restrict__ C, int ldc,
-                  int64_t M, int N, int K, int64_t rows_per_split) {
+                  int64_t M, int N, int K, int64_t rows_per_split, const unsigned* __restrict__ a_amax,
+                  const unsigned* __restrict__ b_amax) {
     extern __shared__ __align__(1024) uint8_t smem[];
     Bars* bars = reinterpret_cast<Bars*>(smem + kStages * 2 * kStageOp);
     const int tid = threadIdx.x, warp = tid >> 5;
@@ -86,13 +90,19 @@ gemm_tn_tc_kernel(const float* __restrict__ A, int lda, const float* __restrict_
     if (warp < 8) {
         const bool isA = warp < 4;
         const int t = tid & 127;
+        // the four columns of this thread are scaled by 2^split_exp(column max) (model.cuh)
+        const int c = (isA ? n0 : k0) + (t & 31) * 4, nc = isA ? N : K;
+        const unsigned* amax = isA ? a_amax : b_amax;
+        float2 fs[4];
+#pragma unroll
+        for (int i = 0; i < 4; ++i) fs[i] = split_factors(c + i < nc ? split_exp(__uint_as_float(amax[c + i])) : 0);
         for (int st = 0; st < nsteps; ++st) {
             const int s = st % kStages;
             const uint32_t use = (uint32_t)(st / kStages);
             mbar_wait_bounded(&bars->empty[s], (use & 1) ^ 1);
             const int64_t m0 = m_begin + (int64_t)st * kBM;
-            if (isA) fill_operand(opA + s * kStageOp, A, lda, m0, m_end, n0, N, t);
-            else fill_operand(opB + s * kStageOp, B, ldb, m0, m_end, k0, K, t);
+            if (isA) fill_operand(opA + s * kStageOp, A, lda, m0, m_end, n0, N, t, fs);
+            else fill_operand(opB + s * kStageOp, B, ldb, m0, m_end, k0, K, t, fs);
             fence_proxy_async_smem();
             mbar_arrive(&bars->full[s]);
         }
@@ -127,11 +137,12 @@ gemm_tn_tc_kernel(const float* __restrict__ A, int lda, const float* __restrict_
         for (int h = 0; h < 2; ++h) {
             const int n = n0 + wg * 64 + (t >> 5) * 16 + ((t & 31) >> 2) + h * 8;
             if (n >= N) continue;
+            const int sa = split_exp(__uint_as_float(a_amax[n]));
 #pragma unroll
-            for (int j = 0; j < 16; ++j) {
+            for (int j = 0; j < 16; ++j) {       // undo the operand scales (exact unless the result leaves fp32's range)
                 const int k = k0 + 8 * j + 2 * (t & 3);
-                if (k < K) atomicAdd(C + (int64_t)n * ldc + k, acc[4 * j + 2 * h]);
-                if (k + 1 < K) atomicAdd(C + (int64_t)n * ldc + k + 1, acc[4 * j + 2 * h + 1]);
+                if (k < K) atomicAdd(C + (int64_t)n * ldc + k, split_unscale(acc[4 * j + 2 * h], -(sa + split_exp(__uint_as_float(b_amax[k])))));
+                if (k + 1 < K) atomicAdd(C + (int64_t)n * ldc + k + 1, split_unscale(acc[4 * j + 2 * h + 1], -(sa + split_exp(__uint_as_float(b_amax[k + 1])))));
             }
         }
     }
@@ -157,6 +168,10 @@ void launch_gemm_tn_tc(const float* A, int lda, const float* B, int ldb, float* 
         P2S_CUDA(cudaFuncSetAttribute(gemm_tn_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmem));
         attr = true;
     }
+    static thread_local DevBuf amax;
+    unsigned* a_amax = amax.as<unsigned>((size_t)N + K);
+    launch_absmax_cols(A, lda, M, N, a_amax, st);
+    launch_absmax_cols(B, ldb, M, K, a_amax + N, st);
     int dev = 0, sms = 132;
     P2S_CUDA(cudaGetDevice(&dev));
     P2S_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
@@ -167,7 +182,7 @@ void launch_gemm_tn_tc(const float* A, int lda, const float* B, int ldb, float* 
     int64_t rows = cdiv(cdiv(M, splits), kBM) * kBM;
     splits = cdiv(M, rows);
     dim3 grid((unsigned)cdiv(N, 128), (unsigned)cdiv(K, 128), (unsigned)splits);
-    P2S_LAUNCH(gemm_tn_tc_kernel, grid, 512, kSmem, st, A, lda, B, ldb, C, ldc, M, N, K, rows);
+    P2S_LAUNCH(gemm_tn_tc_kernel, grid, 512, kSmem, st, A, lda, B, ldb, C, ldc, M, N, K, rows, a_amax, a_amax + N);
 }
 
 }  // namespace p2s

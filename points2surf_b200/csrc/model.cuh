@@ -72,7 +72,7 @@ uint8_t* fc_tc_pack(const Layer& L, std::vector<void*>& allocs);
 void fc_tc_init();
 void launch_fc_tc(const float* A, int lda, const uint8_t* Wimg, const float* bias, float* C, int ldc,
                   int64_t M, int N, int K, bool relu, cudaStream_t st, int pack_img = 0, const float* in_bias = nullptr,
-                  bool in_relu = false);
+                  bool in_relu = false, const int* a_exp = nullptr, const int* w_exp = nullptr);
 uint8_t* fc_tc_pack_raw(const float* W, int N, int K, std::vector<void*>& allocs);
 size_t fc_tc_a_image_bytes(int64_t M, int K);
 void launch_pack_a(const float* A, int lda, int64_t M, int K, const float* in_bias, bool in_relu, uint8_t* img, cudaStream_t st);
@@ -81,6 +81,34 @@ void launch_fc_tc_img(const uint8_t* Aimg, const uint8_t* Wimg, const float* bia
 bool gemm_nt_tc_ok(const float* A, int lda, const float* C, int ldc, int64_t M, int N, int K);
 void launch_gemm_nt_tc(const float* A, int lda, const float* W, const float* bias, float* C, int ldc, int64_t M, int N,
                        int K, bool relu, cudaStream_t st);
+// split_exp (below) of every row of X[rows][cols] (out[rows])
+void launch_split_exp_rows(const float* X, int ld, int64_t rows, int cols, int* out, cudaStream_t st);
+// max |x| of every column of X[rows][cols] as float bits (out[cols], zeroed here; cols % 4 == 0, ld % 4 == 0,
+// X 16-byte aligned)
+void launch_absmax_cols(const float* X, int ld, int64_t rows, int cols, unsigned* out, cudaStream_t st);
+
+// ---- power-of-two operand scaling of the split-precision training GEMMs (fc_tc.cu, gemm_tn_tc.cu)
+// hi = fp16(x), lo = fp16(x - hi) keep ~22 bits of x only while both are fp16 normal numbers.  The training operands are
+// often far outside that range (the backward pass's dZ shrinks like 1 / batch), so every row (gemm_nt) or column (gemm_tn)
+// of an operand is multiplied by 2^s before the split, with s chosen from its largest magnitude `amax` so that the
+// scaled maximum lies in [2^15, 65504].  Each output element is a sum over one row / column pair, so the scales factor
+// out and the epilogue multiplies by 2^-(s_a + s_b).  An element ~2^-40 below its row's maximum keeps nothing but its
+// fp16-subnormal part (half-spacing 2^-25 at a scaled maximum >= 2^15).
+__device__ __forceinline__ int split_exp(float amax) {
+    if (!(amax > 0.f) || !(amax <= 3.4028235e38f)) return 0;      // zero rows; inf / nan propagate unscaled
+    int e;
+    const float f = frexpf(amax, &e);                            // amax = f 2^e, f in [0.5, 1)
+    return f * 65536.f > 65504.f ? 15 - e : 16 - e;              // s in [-113, 164]
+}
+// x 2^s without overflow of the factor: two exact power-of-two multiplications (|s| / 2 <= 82)
+__device__ __forceinline__ float2 split_factors(int s) {
+    const int h = s / 2;
+    return make_float2(__int_as_float((127 + h) << 23), __int_as_float((127 + s - h) << 23));
+}
+// x 2^e rounded once (the epilogue's unscaling): one multiplication while 2^e is a normal float
+__device__ __forceinline__ float split_unscale(float x, int e) {
+    return (e >= -126 && e <= 127) ? x * __int_as_float((127 + e) << 23) : scalbnf(x, e);
+}
 // meshdist.cu
 void mesh_sample(const float* verts, int64_t V, const int32_t* faces, int64_t F, int64_t n, uint64_t seed,
                  float* samples, int32_t* face_ids, cudaStream_t st);

@@ -254,3 +254,166 @@ def test_training_loop_mirror_on_gpu(tmp_path):
     hist = p2s_train.points_to_surf_train(opt)
     assert len([h for h in hist if h[0] == 'train']) == 8 and all(np.isfinite(h[3]).all() for h in hist)
     assert (tmp_path / 'models' / 'test_model.pth').exists()
+
+
+# ---- per-element accuracy of the training GEMMs at every operand scale (oracle/split_gemm.py states the bound:
+# |C - C_f64| <= gamma_K sum_k |a_k b_k| + 2^-40 K max|a| max|b|, gamma_K the fp32 dot-product bound).  The tensor-core
+# cases run in this process; the same cases run on the fp32 FMA kernels in a subprocess with P2S_TRAIN_GEMM_FP32=1
+# (read once per process), and must meet the same bound.
+_SCALES = {'2^-30': 2.0 ** -30, '2^-20': 2.0 ** -20, '2^-14': 2.0 ** -14, '1': 1.0, '2^14': 2.0 ** 14, '2^17': 2.0 ** 17}
+
+
+def _pow2(shape, lo, hi, seed):
+    g = torch.Generator().manual_seed(seed)
+    return torch.pow(2.0, torch.randint(lo, hi, shape, generator=g).float()).to(DEV)
+
+
+def _gemm_case(name):
+    """-> (kind, operands, accumulate-into or None) of one named case; kind 'nt': A [M,K], W [N,K]; 'tn': A [M,N], B [M,K]."""
+    kind, rest = name.split(':')
+    if rest.startswith('scale'):
+        s = _SCALES[rest.split('=')[1]]
+        if kind == 'nt':
+            return kind, (rnd(4096, 1024, seed=40, scale=s), rnd(512, 1024, seed=41, scale=s)), None
+        return kind, (rnd(8192, 256, seed=42, scale=s), rnd(8192, 128, seed=43, scale=s)), None
+    if rest == 'mixed':          # rows / columns of one operand spread over 2^-30 .. 2^17
+        if kind == 'nt':
+            return kind, (rnd(4096, 256, seed=44) * _pow2((4096, 1), -30, 18, 45), rnd(256, 256, seed=46) * _pow2((1, 256), -30, 18, 47)), None
+        return kind, (rnd(8192, 128, seed=48) * _pow2((1, 128), -30, 18, 49), rnd(8192, 128, seed=50) * _pow2((8192, 1), -30, 18, 51)), None
+    if rest == 'zero_tiny':      # all-zero and all-tiny rows (nt: rows of A / W; tn: columns of A / B)
+        A, B = rnd(4096, 128, seed=52, scale=2.0 ** -16), rnd(4096 if kind == 'tn' else 128, 128, seed=53)
+        if kind == 'nt':
+            A[:64], A[64:128], B[:4], B[4:8] = 0.0, A[64:128] * 2.0 ** -40, 0.0, B[4:8] * 2.0 ** -40
+        else:      # (tiny x tiny stays a normal fp32 number: the bound is about the kernels, not fp32's range)
+            A[:, :8], A[:, 8:16], B[:, :4], B[:, 4:8] = 0.0, A[:, 8:16] * 2.0 ** -40, 0.0, B[:, 4:8] * 2.0 ** -40
+        return kind, (A, B), None
+    # training shapes: dZ ~ 2^-16 (a batch mean over ~1000 queries), weights ~ 0.05, activations >= 0 (post ReLU)
+    dims = [int(x) for x in rest.split('x')[:3]]
+    acc = rest.endswith('acc')
+    if kind == 'nt':
+        M, N, K = dims
+        return kind, (rnd(M, K, seed=54, scale=2.0 ** -16), rnd(N, K, seed=55, scale=0.05)), None
+    M, N, K = dims
+    return kind, (rnd(M, N, seed=56, scale=2.0 ** -16), rnd(M, K, seed=57).abs()), (rnd(N, K, seed=58, scale=1e-3) if acc else None)
+
+
+_GEMM_CASES = ([k + ':scale=' + s for k in ('nt', 'tn') for s in _SCALES] + ['nt:mixed', 'tn:mixed', 'nt:zero_tiny', 'tn:zero_tiny'] +
+               ['nt:300x64x64', 'nt:70000x64x1024', 'nt:20000x128x128', 'nt:4096x4096x256', 'nt:1024x512x1024',
+                'tn:128x64x64', 'tn:4096x1024x128', 'tn:204800x1024x128x_acc', 'tn:300000x64x64x_acc', 'tn:8192x4096x64',
+                'tn:20000x128x1024'])
+
+
+def _gemm_excess(name):
+    from oracle import split_gemm
+    p = CudaPrims()
+    kind, (X, Y), acc = _gemm_case(name)
+    if kind == 'nt':
+        got, exact, bound = p.gemm_nt(X, Y), X.double() @ Y.double().t(), split_gemm.bound_nt(X, Y)
+    else:
+        exact = X.double().t() @ Y.double()
+        if acc is None:
+            got, bound = p.gemm_tn(X, Y), split_gemm.bound_nt(X.t(), Y.t())
+        else:
+            got = p.gemm_tn(X, Y, out=acc.clone())
+            exact, bound = exact + acc.double(), split_gemm.bound_nt(X.t(), Y.t(), extra=acc)
+    return split_gemm.excess(got, exact, bound)
+
+
+@pytest.mark.parametrize('name', _GEMM_CASES)
+def test_gemm_per_element_bound(name):
+    e = _gemm_excess(name)
+    print(name, 'max error / bound %.3g' % e)
+    assert e <= 1.0, (name, e)
+
+
+_FP32_GEMM_SCRIPT = r'''
+import json, sys
+sys.path[:0] = [%r, %r]
+import test_gpu_train as t
+print('EXCESS ' + json.dumps({n: t._gemm_excess(n) for n in t._GEMM_CASES}))
+'''
+
+
+def test_gemm_per_element_bound_fp32_fma_kernels():
+    import json
+    import os
+    import subprocess
+    import sys
+    here = os.path.dirname(os.path.abspath(__file__))
+    env = dict(os.environ, P2S_TRAIN_GEMM_FP32='1')
+    r = subprocess.run([sys.executable, '-c', _FP32_GEMM_SCRIPT % (os.path.dirname(here), here)], env=env, capture_output=True,
+                       text=True, timeout=1200)
+    assert r.returncode == 0, (r.stdout[-2000:], r.stderr[-2000:])
+    ex = json.loads([l for l in r.stdout.splitlines() if l.startswith('EXCESS ')][-1][7:])
+    print({k: round(v, 4) for k, v in ex.items()})
+    assert set(ex) == set(_GEMM_CASES) and all(v <= 1.0 for v in ex.values()), ex
+
+
+# ---- one training step at a realistic batch: gradients shrink like 1 / batch, so batch 1024 puts dZ where a
+# split-precision GEMM without operand scaling loses most of its bits.  P and S are small to keep the float64 CPU oracle
+# short (the gradient magnitudes follow the batch, not P or S).  The tensor-core step must stay within twice the error of
+# the same step on the fp32 FMA GEMMs (P2S_TRAIN_GEMM_FP32=1, subprocess), plus a floor of 1e-2 relative L2: the split
+# products carry ~3 * 2^-22 relative error each (12x fp32's unit roundoff), and gradients that come out of cancelling
+# sums (BatchNorm biases: column sums of dZ) magnify that to a few 1e-3 even with well-scaled operands.  Without operand
+# scaling the worst tensors sit at 0.11 - 0.18.
+_BIG_B, _BIG_P, _BIG_S, _BIG_FLOOR = 1024, 64, 128, 1e-2
+_VARIANTS = ['vanilla', 'max', 'uniform']
+
+
+def _big_step_grads(variant):
+    v = synth.VARIANTS[variant]
+    sd = synth.make_state_dict(variant, seed=TRAIN_SEEDS[variant])
+    batch = make_train_batch(_BIG_B, _BIG_P, _BIG_S, seed=11)
+    ts = TrainStep({k: t.to(DEV) for k, t in sd.items()}, v['use_point_stn'], v['shared_transformer'], points_per_patch=_BIG_P,
+                   sub_sample_size=_BIG_S, lr=0.01, momentum=0.9)
+    ts.step(_cuda_batch(batch))
+    return {k: t.detach().cpu().clone() for k, t in ts.named_gradients().items()}
+
+
+_FP32_STEP_SCRIPT = r'''
+import sys, torch
+sys.path[:0] = [%r, %r]
+import test_gpu_train as t
+torch.save({v: t._big_step_grads(v) for v in t._VARIANTS}, %r)
+'''
+
+
+@pytest.fixture(scope='module')
+def fp32_big_step_grads(tmp_path_factory):
+    import os
+    import subprocess
+    import sys
+    here = os.path.dirname(os.path.abspath(__file__))
+    out = str(tmp_path_factory.mktemp('fp32_step') / 'grads.pt')
+    env = dict(os.environ, P2S_TRAIN_GEMM_FP32='1')
+    r = subprocess.run([sys.executable, '-c', _FP32_STEP_SCRIPT % (os.path.dirname(here), here, out)], env=env, capture_output=True,
+                       text=True, timeout=1200)
+    assert r.returncode == 0, (r.stdout[-2000:], r.stderr[-2000:])
+    return torch.load(out)
+
+
+def _rel_l2(grads, ref):
+    nscale = max(float(r.double().norm()) for r in ref.values())
+    per, num, den = {}, 0.0, 0.0
+    for name, r in ref.items():
+        d = grads[name].double().reshape(-1) - r.double().reshape(-1)
+        per[name] = float(d.norm()) / (float(r.double().norm()) + 1e-3 * nscale)
+        num += float((d * d).sum())
+        den += float((r.double() ** 2).sum())
+    return per, (num / den) ** 0.5
+
+
+@pytest.mark.parametrize('variant', _VARIANTS)
+def test_train_step_batch_1024_as_accurate_as_fp32(variant, fp32_big_step_grads):
+    v = synth.VARIANTS[variant]
+    sd = synth.make_state_dict(variant, seed=TRAIN_SEEDS[variant])
+    ref = train_oracle.train_iteration(sd, make_train_batch(_BIG_B, _BIG_P, _BIG_S, seed=11), v['use_point_stn'],
+                                       v['shared_transformer'], lr=0.01, momentum=0.9, dtype=torch.float64)['grads']
+    per_tc, glob_tc = _rel_l2(_big_step_grads(variant), ref)
+    per_fp, glob_fp = _rel_l2(fp32_big_step_grads[variant], ref)
+    worst = max(per_tc, key=lambda n: per_tc[n] - 2 * per_fp[n])
+    print(variant, 'global rel-L2: tensor cores %.3g, fp32 %.3g; worst tensor %s: %.3g vs %.3g' %
+          (glob_tc, glob_fp, worst, per_tc[worst], per_fp[worst]))
+    bad = {n: (round(per_tc[n], 5), round(per_fp[n], 5)) for n in per_tc if per_tc[n] > 2 * per_fp[n] + _BIG_FLOOR}
+    assert not bad, bad
+    assert glob_tc <= 2 * glob_fp + _BIG_FLOOR, (glob_tc, glob_fp)
