@@ -255,6 +255,56 @@ int p2s_range_scan_dev(const float* verts, int64_t V, const int32_t* faces, int6
                        const p2s_scan_config* cfg, uint64_t seed, float* pts_noisy, float* pts_clean, int32_t* face_ids,
                        int64_t cap, int32_t* hits_per_scan, int64_t* total_host, void* stream);
 
+/* ------------------------------------------------------------------ mesh cleaning -------------- */
+/* The repair of make_dataset.py:_clean_mesh (make_dataset.py:383-413: trimesh's process, remove_degenerate_faces,
+ * remove_duplicate_faces, fill_holes, fix_inversion / fix_normals / fix_winding) without the file I/O and the accept /
+ * reject decision.  In this order:
+ *   1. non-finite: faces that reference a vertex with a non-finite coordinate are dropped.
+ *   2. weld (tol.merge = 1e-8): two finite vertices merge iff llround(double(x) * 1e8) is equal for all three
+ *      coordinates; the merged vertex keeps the coordinates of its lowest input index.  A finite |coordinate| >= 9e10
+ *      is an error (the key overflows int64).
+ *   3. degenerate: a face with two equal (welded) indices, or whose float64 altitude over its longest edge
+ *      (2 area / longest edge) is <= 1e-8, is dropped.
+ *   4. duplicate: faces with the same vertex set, in either orientation; the first is kept.
+ *   5. edges: the faces on every undirected edge are counted.  Watertight: every edge has exactly two faces.  The winding
+ *      is consistent iff the two faces of every two-face edge traverse it in opposite directions.
+ *   6. holes: a boundary loop (a closed chain of one-face edges through vertices of boundary degree 2) of 3 edges gets
+ *      one face, of 4 edges two faces split along the diagonal through the loop's lowest vertex.  Fill faces run
+ *      opposite to the loop's edge from its lowest vertex v to v's lower boundary neighbour.  Longer loops and loops
+ *      through a vertex of boundary degree != 2 stay open.  Step 5 is redone.
+ *   7. orientation, only when the winding is inconsistent after 6 (a closed, consistent, all-inverted mesh is not
+ *      flipped): components are connected over two-face edges.  A component is orientable iff some choice of face
+ *      flips makes all its two-face edges consistent; its faces are then reversed ((a,b,c) -> (c,b,a)) relative to its
+ *      lowest face, and the whole component again when its float64 signed volume sum det(v0,v1,v2) / 6 is < 0.
+ *      Non-orientable components, and faces without a two-face edge, are left as they came.
+ *   8. vertices no output face uses are dropped.
+ * Output order: vertices ascending by their lowest merged input index; faces in input order without the dropped ones,
+ * then the fill faces ordered by their loop's lowest vertex.  A clean mesh comes back bit-identical.
+ * Deviations from trimesh: first-occurrence vertex order (trimesh: hash order; some versions also reorder faces when
+ * removing duplicates); the quad diagonal is fixed by the lowest vertex (trimesh: networkx cycle_basis order); loops
+ * through non-manifold vertices are not filled; vertices referenced only by dropped faces are dropped here (trimesh
+ * keeps them until the mesh is reloaded); the orientation of non-orientable components and of open components with
+ * signed volume exactly 0 is not pinned.
+ *   verts [V,3] fp32, faces [F,3] int32 (every index in [0, V), else an error)
+ *   verts_out [vcap,3] fp32, faces_out [fcap,3] int32: vcap >= V and fcap >= 2 F always suffice; a smaller capacity
+ *   that turns out too small is an error, not a truncation.
+ * Bitwise deterministic (the signed volumes are reduced in a fixed order, no float atomics).  sync: report read-back. */
+typedef struct {
+    int64_t vertices_in, faces_in, vertices_out, faces_out;
+    int64_t merged_vertices;               /* input vertices welded onto a lower index */
+    int64_t unreferenced_vertices;         /* welded vertices (non-finite ones included) no output face uses */
+    int64_t nonfinite_faces, degenerate_faces, duplicate_faces;
+    int64_t boundary_edges, nonmanifold_edges;    /* after hole filling */
+    int64_t holes_filled, faces_added;
+    int64_t components, nonorientable_components, faces_reversed;   /* of step 7; 0 when it did not run */
+    int32_t watertight_before, winding_consistent_before;            /* after hole filling, before step 7 */
+    int32_t watertight, winding_consistent;                          /* of the output */
+    double volume;                                                   /* float64 signed volume of the output */
+} p2s_clean_report;
+
+int p2s_mesh_clean_dev(const float* verts, int64_t V, const int32_t* faces, int64_t F, float* verts_out, int64_t vcap,
+                       int32_t* faces_out, int64_t fcap, p2s_clean_report* report_host, void* stream);
+
 /* ------------------------------------------------------------------ training-step primitives --- */
 /* Row a14 (SURVEY.md section 8a): loss + backward + SGD of source/points_to_surf_train.py:441-461,537-563 with the
  * train-mode BatchNorm of source/points_to_surf_model.py.  Activations are row-major [rows, C] fp32.  The host side

@@ -25,6 +25,15 @@ class ScanConfig(C.Structure):
                 ('max_distance', C.c_float), ('noise_mu', C.c_float), ('noise_sigma', C.c_float), ('first_scan', C.c_int32)]
 
 
+class CleanReport(C.Structure):
+    _fields_ = [(n, C.c_int64) for n in (
+        'vertices_in', 'faces_in', 'vertices_out', 'faces_out', 'merged_vertices', 'unreferenced_vertices',
+        'nonfinite_faces', 'degenerate_faces', 'duplicate_faces', 'boundary_edges', 'nonmanifold_edges', 'holes_filled',
+        'faces_added', 'components', 'nonorientable_components', 'faces_reversed')] + \
+        [(n, C.c_int32) for n in ('watertight_before', 'winding_consistent_before', 'watertight', 'winding_consistent')] + \
+        [('volume', C.c_double)]
+
+
 PRECISION_FP32, PRECISION_TC = 0, 1
 SUBSAMPLE_WEIGHTED, SUBSAMPLE_UNIFORM = 0, 1
 
@@ -82,6 +91,7 @@ SIGNATURES = {
     'p2s_mesh_signed_distance_dev': (C.c_int, [_vp, _i64, _vp, _i64, _vp, _i64, _vp, _vp, _vp, _vp]),
     'p2s_range_scan_dev': (C.c_int, [_vp, _i64, _vp, _i64, _vp, _i64, C.POINTER(ScanConfig), C.c_uint64, _vp, _vp, _vp,
                                      _i64, _vp, C.POINTER(_i64), _vp]),
+    'p2s_mesh_clean_dev': (C.c_int, [_vp, _i64, _vp, _i64, _vp, _i64, _vp, _i64, C.POINTER(CleanReport), _vp]),
 }
 
 _lib = None

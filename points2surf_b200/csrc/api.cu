@@ -481,6 +481,14 @@ int p2s_range_scan_dev(const float* verts, int64_t V, const int32_t* faces, int6
     });
 }
 
+int p2s_mesh_clean_dev(const float* verts, int64_t V, const int32_t* faces, int64_t F, float* verts_out, int64_t vcap,
+                       int32_t* faces_out, int64_t fcap, p2s_clean_report* report_host, void* stream) {
+    return guarded([&] {
+        P2S_CHECK((verts || V == 0) && (faces || F == 0) && report_host, "null argument");
+        mesh_clean(verts, V, faces, F, verts_out, vcap, faces_out, fcap, report_host, as_stream(stream));
+    });
+}
+
 // ---- training-step primitives (train_ops.cu)
 #define P2S_OP(name, params, ...)                                   \
     int name params { return guarded([&] { __VA_ARGS__; }); }

@@ -121,6 +121,9 @@ void mesh_signed_distance(const float* verts, int64_t V, const int32_t* faces, i
 void range_scan(const float* verts, int64_t V, const int32_t* faces, int64_t F, const double* poses, int64_t S,
                 const p2s_scan_config& cfg, uint64_t seed, float* pts_noisy, float* pts_clean, int32_t* face_ids,
                 int64_t cap, int32_t* hits_per_scan, int64_t* total_host, cudaStream_t st);
+// meshclean.cu
+void mesh_clean(const float* verts, int64_t V, const int32_t* faces, int64_t F, float* verts_out, int64_t vcap,
+                int32_t* faces_out, int64_t fcap, p2s_clean_report* report, cudaStream_t st);
 // gemm_tn_tc.cu
 bool gemm_tn_tc_ok(const float* A, int lda, const float* B, int ldb, int64_t M, int N, int K);
 void launch_gemm_tn_tc(const float* A, int lda, const float* B, int ldb, float* C, int ldc, int64_t M, int N, int K,

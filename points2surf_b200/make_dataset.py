@@ -1,11 +1,14 @@
-"""Two stages of the reference's make_dataset.py for every mesh in 03_meshes, on the GPU:
+"""The reference's make_dataset.py, with its mesh work on the GPU:
+  - convert_meshes, clean_meshes (csrc/meshclean.cu), normalize_meshes: 00_base_meshes -> 01_base_meshes_ply ->
+    02_meshes_cleaned -> 03_meshes;
   - with --scan, the input point clouds 04_pts (sample_blensor, make_dataset.py:242-380): simulated time-of-flight scans
     (csrc/scan.cu) instead of Blender / BlenSor, with the reference's scan poses and noise levels;
   - the training targets 05_query_pts / 05_query_dist (and optionally 05_query_vis) of the query-point stage
-    (make_dataset.py:447-538), with the signed distances of csrc/meshsdf.cu.
-Cleaning, normalisation and dataset splits are not part of this module.
+    (make_dataset.py:447-538), with the signed distances of csrc/meshsdf.cu;
+  - clean_up_broken_inputs, make_dataset_splits and make_dataset, which runs all of it (--from_base_meshes).
 
     python -m points2surf_b200.make_dataset DATASET_DIR [--scan] [--num_query_pts 2000] [--far_query_pts_ratio 0.5] [--debug]
+    python -m points2surf_b200.make_dataset DATASET_DIR --from_base_meshes [--num_query_pts 2000]
 
 From DATASET_DIR/settings.ini: patch_radius = (1 + epsilon) / grid_resolution (make_dataset.py:760); with --scan also
 num_scans_per_mesh_min/max, scanner_noise_sigma_min/max and only_for_evaluation (make_dataset.py:809-815)."""
@@ -13,6 +16,8 @@ import argparse
 import configparser
 import hashlib
 import os
+import random
+import shutil
 import sys
 
 import numpy as np
@@ -165,6 +170,216 @@ def sample_blensor(base_dir, dataset_dir, blensor_bin, dir_in, dir_out_raw, dir_
         _scan_and_save_pts(file_in_mesh, file_pts, file_vis, file_hits, noise_sigma, locations, rotations, min_pts_size)
 
 
+def convert_meshes(in_dir_abs, out_dir_abs, target_file_type: str, num_processes=8):
+    """make_dataset.py:21-68: every .off / .ply / .obj / .stl under in_dir_abs (recursively) whose output is missing or
+    older -> out_dir_abs/<name><target_file_type> as binary PLY (mesh_io.read_mesh; polygons fan-triangulated).  The
+    faces are written as read, without welding: an STL stays a triangle soup until the clean stage welds it.  Files
+    that fail to parse are reported and skipped, like the reference's except branches.  `num_processes` is accepted
+    and ignored."""
+    if target_file_type != '.ply':
+        raise ValueError('only .ply output is supported, got %s' % target_file_type)
+    os.makedirs(out_dir_abs, exist_ok=True)
+    mesh_files = []
+    for root, dirs, files in os.walk(in_dir_abs, topdown=True):
+        for name in files:
+            mesh_files.append(os.path.join(root, name))
+    mesh_files = [f for f in mesh_files if f[-4:] in ('.off', '.ply', '.obj', '.stl')]
+    for f in mesh_files:
+        file_out = os.path.join(out_dir_abs, os.path.basename(f)[:-4] + target_file_type)
+        if not sdf._call_necessary([f], [file_out]):
+            continue
+        try:
+            verts, faces = mesh_io.read_mesh(f)
+        except (AttributeError, IndexError, ValueError, NameError, UnicodeDecodeError, AssertionError) as e:
+            print(e)
+            continue
+        mesh_io.write_ply(file_out, verts, faces)
+
+
+def _accept_cleaned(report, num_faces, num_max_faces=None, enforce_solid=True):
+    """The decisions of _clean_mesh (make_dataset.py:395-413) on a p2s_mesh_clean report, in the reference's order:
+    with enforce_solid reject if not watertight, if the winding is still inconsistent, or unless is_volume (watertight,
+    consistent, finite, volume > 0); then write only if num_faces < num_max_faces."""
+    if enforce_solid and not report['watertight']:
+        return False
+    if enforce_solid and not report['winding_consistent']:
+        return False
+    if enforce_solid and not (report['watertight'] and report['winding_consistent'] and np.isfinite(report['volume'])
+                              and report['volume'] > 0.0):
+        return False
+    return num_max_faces is None or num_faces < num_max_faces
+
+
+def _clean_mesh(file_in, file_out, num_max_faces=None, enforce_solid=True):
+    """make_dataset.py:383-413: repair the mesh on the GPU (ops.mesh_clean), then write it as binary PLY if
+    _accept_cleaned accepts the report."""
+    verts, faces = mesh_io.read_mesh(file_in)
+    dev = sdf._device()
+    v, f, report = ops.mesh_clean(torch.from_numpy(np.ascontiguousarray(verts, np.float32)).to(dev),
+                                  torch.from_numpy(np.ascontiguousarray(faces, np.int32)).to(dev))
+    if _accept_cleaned(report, len(f), num_max_faces, enforce_solid):
+        mesh_io.write_ply(file_out, v.cpu().numpy(), f.cpu().numpy())
+
+
+def clean_meshes(base_dir, dataset_dir, dir_in_meshes, dir_out, num_processes, num_max_faces=None, enforce_solid=True):
+    """make_dataset.py:416-444: _clean_mesh for every file in dir_in_meshes whose output is missing or older.
+    `num_processes` is accepted and ignored."""
+    dir_in_abs = os.path.join(base_dir, dataset_dir, dir_in_meshes)
+    dir_out_abs = os.path.join(base_dir, dataset_dir, dir_out)
+    os.makedirs(dir_out_abs, exist_ok=True)
+    for f in [f for f in os.listdir(dir_in_abs) if os.path.isfile(os.path.join(dir_in_abs, f))]:
+        file_in, file_out = os.path.join(dir_in_abs, f), os.path.join(dir_out_abs, f)
+        if sdf._call_necessary([file_in], [file_out]):
+            _clean_mesh(file_in, file_out, num_max_faces, enforce_solid)
+
+
+def normalized_vertices(verts):
+    """make_dataset.py:71-88 on the vertices: None when an extent is 0, else float32((v + t) s) with
+    t = -(min + max) / 2 and s = 1 / max extent, in float64 -- what trimesh's two apply_transform calls compute."""
+    v = np.asarray(verts, np.float64)
+    if len(v) == 0:
+        return None
+    lo, hi = v.min(0), v.max(0)
+    ext = hi - lo
+    if ext.min() == 0.0:
+        return None
+    t = -((lo + hi) * 0.5)
+    s = 1.0 / ext.max()
+    return ((v + t) * s).astype(np.float32)
+
+
+def _normalize_mesh(file_in, file_out):
+    """make_dataset.py:71-88: translate to the origin and scale to the unit cube; nothing is written when the mesh has
+    zero extent along an axis."""
+    verts, faces = mesh_io.read_ply(file_in)
+    v = normalized_vertices(verts if verts is not None else np.zeros((0, 3)))
+    if v is not None:
+        mesh_io.write_ply(file_out, v, faces)
+
+
+def normalize_meshes(base_dir, in_dir, out_dir, dataset_dir, num_processes=1):
+    """make_dataset.py:91-121.  `num_processes` is accepted and ignored."""
+    in_dir_abs = os.path.join(base_dir, dataset_dir, in_dir)
+    out_dir_abs = os.path.join(base_dir, dataset_dir, out_dir)
+    os.makedirs(out_dir_abs, exist_ok=True)
+    for f in [f for f in os.listdir(in_dir_abs) if os.path.isfile(os.path.join(in_dir_abs, f))]:
+        file_in, file_out = os.path.join(in_dir_abs, f), os.path.join(out_dir_abs, f)
+        if sdf._call_necessary([file_in], [file_out]):
+            _normalize_mesh(file_in, file_out)
+
+
+def make_dataset_splits(base_dir, dataset_dir, final_out_dir, seed=42, only_test_set=False, testset_ratio=0.1):
+    """make_dataset.py:541-577, restated exactly: trainset.txt, testset.txt and valset.txt (= the test set) from the .npy
+    files of final_out_dir in os.listdir order, the test set drawn by random.Random(seed).sample."""
+    rnd = random.Random(seed)
+    final_out_dir_abs = os.path.join(base_dir, dataset_dir, final_out_dir)
+    final_output_files = [f for f in os.listdir(final_out_dir_abs)
+                          if os.path.isfile(os.path.join(final_out_dir_abs, f)) and f[-4:] == '.npy']
+    files_dataset = [f[:-8] for f in final_output_files]
+    if len(files_dataset) == 0:
+        raise ValueError('Dataset is empty! {}'.format(final_out_dir_abs))
+    if only_test_set:
+        files_test = files_dataset
+    else:
+        files_test = rnd.sample(files_dataset, max(3, min(int(testset_ratio * len(files_dataset)), 100)))
+    files_train = list(set(files_dataset).difference(set(files_test)))
+    files_test.sort()
+    files_train.sort()
+    file_train_set = os.path.join(base_dir, dataset_dir, 'trainset.txt')
+    file_test_set = os.path.join(base_dir, dataset_dir, 'testset.txt')
+    file_val_set = os.path.join(base_dir, dataset_dir, 'valset.txt')
+    mesh_io.make_dir_for_file(file_test_set)
+    with open(file_test_set, 'w') as text_file:
+        text_file.write('\n'.join(files_test))
+    if not only_test_set:
+        with open(file_train_set, 'w') as text_file:
+            text_file.write('\n'.join(files_train))
+    with open(file_val_set, 'w') as text_file:
+        text_file.write('\n'.join(files_test))   # the test set doubles as the validation set
+
+
+def clean_up_broken_inputs(base_dir, dataset_dir, final_out_dir, final_out_extension, clean_up_dirs,
+                           broken_dir='broken'):
+    """make_dataset.py:580-617, restated exactly: move every file of clean_up_dirs whose stem (the name up to its first
+    '.') has no file in final_out_dir (with final_out_extension, None = any) to broken_dir/<dir>/."""
+    final_out_dir_abs = os.path.join(base_dir, dataset_dir, final_out_dir)
+    final_output_files = [f for f in os.listdir(final_out_dir_abs)
+                          if os.path.isfile(os.path.join(final_out_dir_abs, f)) and
+                          (final_out_extension is None or f[-len(final_out_extension):] == final_out_extension)]
+    if len(final_output_files) == 0:
+        print('Warning: Output dir "{}" is empty'.format(final_out_dir_abs))
+        return
+    final_output_file_stems = set(f.split('.', 1)[0] for f in final_output_files)
+    for clean_up_dir in clean_up_dirs:
+        dir_abs = os.path.join(base_dir, dataset_dir, clean_up_dir)
+        if not os.path.isdir(dir_abs):
+            continue
+        dir_files = [f for f in os.listdir(dir_abs) if os.path.isfile(os.path.join(dir_abs, f))]
+        dir_files_without_final_output = [f for f in dir_files if f.split('.', 1)[0] not in final_output_file_stems]
+        broken_dir_abs = os.path.join(base_dir, dataset_dir, broken_dir, clean_up_dir)
+        for f in dir_files_without_final_output:
+            os.makedirs(broken_dir_abs, exist_ok=True)
+            shutil.move(os.path.join(dir_abs, f), os.path.join(broken_dir_abs, f))
+
+
+DIRS_TO_CLEAN = ['00_base_meshes', '01_base_meshes_ply', '02_meshes_cleaned', '03_meshes',
+                 '04_pts', '04_pts_raw', '04_pts_vis', '04_blensor_py', '04_locations', '04_rotations',
+                 '05_patch_dists', '05_patch_ids', '05_query_dist', '05_query_pts',
+                 '05_patch_ids_grid', '05_query_pts_grid', '05_query_dist_grid',
+                 '06_poisson_rec', '06_mc_gt_recon', '06_poisson_rec_gt_normals',
+                 '06_normals', '06_normals/pts', '06_dist_from_p_normals']
+
+
+def make_dataset(dataset_name: str, blensor_bin: str, base_dir: str, num_processes=7, seed=42,
+                 num_query_points_per_shape=2000):
+    """make_dataset.py:731-850: 00_base_meshes -> 01_base_meshes_ply -> 02_meshes_cleaned -> 03_meshes -> 04_pts ->
+    05_query_pts / 05_query_dist -> trainset / testset / valset.txt, with the reference's stage order, settings,
+    clean-ups and splits.  `blensor_bin` and `num_processes` are accepted and ignored (the scans are simulated on the
+    GPU, and the shapes run one after the other)."""
+    dataset_dir = dataset_name
+    config_file = os.path.join(base_dir, dataset_dir, 'settings.ini')
+    if not os.path.isfile(config_file):
+        raise ValueError('no settings.ini in %s' % os.path.join(base_dir, dataset_dir))
+    config = configparser.ConfigParser()
+    config.read(config_file)
+    print('Processing dataset: ' + config_file)
+    general = config['general']
+    only_for_evaluation = bool(int(general['only_for_evaluation']))
+    patch_radius = (1.0 + int(general['epsilon'])) / int(general['grid_resolution'])
+
+    def clean_up(final_out_dir, ext):
+        clean_up_broken_inputs(base_dir, dataset_dir, final_out_dir, ext, DIRS_TO_CLEAN, 'broken')
+
+    clean_up('00_base_meshes', None)
+    print('### convert base meshes to ply')
+    convert_meshes(os.path.join(base_dir, dataset_dir, '00_base_meshes'),
+                   os.path.join(base_dir, dataset_dir, '01_base_meshes_ply'), '.ply', num_processes)
+    clean_up('01_base_meshes_ply', '.ply')
+    print('### clean mesh')
+    clean_meshes(base_dir, dataset_dir, '01_base_meshes_ply', '02_meshes_cleaned', num_processes,
+                 num_max_faces=None if only_for_evaluation else 50000, enforce_solid=not only_for_evaluation)
+    clean_up('02_meshes_cleaned', '.ply')
+    print('### scale and translate mesh')
+    normalize_meshes(base_dir, '02_meshes_cleaned', '03_meshes', dataset_dir, num_processes)
+    print('### sample with Blensor')
+    sample_blensor(base_dir, dataset_dir, blensor_bin, '03_meshes', '04_pts_raw', '04_pts', '04_pts_vis', '04_pcd',
+                   '04_blensor_py', '04_locations', '04_rotations', int(general['num_scans_per_mesh_min']),
+                   int(general['num_scans_per_mesh_max']), num_processes,
+                   min_pts_size=0 if only_for_evaluation else 100,
+                   scanner_noise_sigma_min=float(general['scanner_noise_sigma_min']),
+                   scanner_noise_sigma_max=float(general['scanner_noise_sigma_max']))
+    clean_up('04_pts', '.xyz.npy')
+    if not only_for_evaluation:
+        print('### make query points, calculate signed distances')
+        get_query_pts_dist_ms(base_dir, dataset_dir, '03_meshes', '05_query_pts', '05_query_dist', '05_query_vis',
+                              patch_radius, num_query_pts=num_query_points_per_shape, far_query_pts_ratio=0.5,
+                              signed_distance_batch_size=500, num_processes=num_processes, debug=True)
+        print('### statistics and clean up')
+        clean_up('05_query_dist', '.npy')
+    make_dataset_splits(base_dir, dataset_dir, '04_pts' if only_for_evaluation else '05_query_pts', seed=seed,
+                        only_test_set=only_for_evaluation, testset_ratio=0.1)
+
+
 def main(argv=None):
     parser = argparse.ArgumentParser(description='Query points and ground-truth signed distances (05_query_pts, '
                                                  '05_query_dist) for the meshes in DATASET_DIR/03_meshes, and with '
@@ -175,8 +390,15 @@ def main(argv=None):
     parser.add_argument('--debug', action='store_true', help='also write coloured query points to 05_query_vis')
     parser.add_argument('--scan', action='store_true',
                         help='first scan the meshes into the input point clouds 04_pts (simulated time-of-flight scans)')
+    parser.add_argument('--from_base_meshes', action='store_true',
+                        help='run the whole make_dataset from DATASET_DIR/00_base_meshes (convert, clean, normalise, '
+                             'scan, query points, splits); --scan, --debug and --far_query_pts_ratio do not apply')
     args = parser.parse_args(argv)
     dataset = os.path.abspath(args.dataset_dir)
+    if args.from_base_meshes:
+        make_dataset(os.path.basename(dataset), None, os.path.dirname(dataset),
+                     num_query_points_per_shape=args.num_query_pts)
+        return
     config_file = os.path.join(dataset, 'settings.ini')
     if not os.path.isfile(config_file):
         raise SystemExit('no settings.ini in %s (needs [general] grid_resolution and epsilon)' % dataset)

@@ -2,6 +2,7 @@
   write_off   -- same text layout as source/base/mesh_io.py:79-130 (OFF / COFF)
   write_ply   -- binary little-endian PLY (what trimesh's exporter writes for source/sdf.py:225-228,285)
   read_ply    -- reader for the PLY files this module and trimesh write (ascii or binary_little_endian)
+  read_off / read_obj / read_stl -- the other input formats of make_dataset.convert_meshes; read_mesh dispatches
 """
 import os
 
@@ -118,35 +119,74 @@ def read_ply(file_path):
     return verts, faces
 
 
+def _fan(polygons):
+    """Polygons (lists of vertex indices) -> triangles [F,3] int32, fans from each polygon's first vertex.  For a quad
+    (a, b, c, d) this gives (a, b, c), (a, c, d): the triangles of trimesh's triangulate_quads."""
+    tris = [(p[0], p[k], p[k + 1]) for p in polygons for k in range(1, len(p) - 1)]
+    return np.array(tris, dtype=np.int32).reshape(-1, 3)
+
+
 def read_off(file_path):
-    """OFF / COFF text files as written by write_off -> (vertices [V,3] float32, faces [F,3] int32)."""
+    """OFF / COFF text files -> (vertices [V,3] float32, faces [F,3] int32); polygon faces are fan-triangulated and
+    per-vertex / per-face colours are skipped."""
     with open(file_path) as fp:
-        tokens = fp.read().split()
-    head = tokens[0]
-    if head not in ('OFF', 'COFF'):
+        lines = [ln.split('#', 1)[0].split() for ln in fp]
+    lines = [t for t in lines if t]
+    head = lines[0]
+    if not head[0].endswith('OFF'):
         raise ValueError('not an OFF file: %s' % file_path)
-    nv, nf = int(tokens[1]), int(tokens[2])
-    per_v = (len(tokens) - 4 - 4 * nf) // max(nv, 1) if head == 'COFF' else 3   # xyz + colour components
-    pos = 4
-    vals = np.array(tokens[pos:pos + nv * per_v], dtype=np.float64).reshape(nv, per_v)
-    verts = vals[:, :3].astype(np.float32)
-    pos += nv * per_v
-    faces = np.zeros((nf, 3), np.int32)
-    for i in range(nf):
-        n = int(tokens[pos])
-        if n != 3:
-            raise ValueError('non-triangular face in %s' % file_path)
-        faces[i] = [int(t) for t in tokens[pos + 1:pos + 4]]
-        pos += 1 + n
-        # optional per-face colours are not written by write_off for triangle meshes
-    return verts, faces
+    counts = head[1:] if len(head) > 1 else lines[1]
+    pos = 1 if len(head) > 1 else 2
+    nv, nf = int(counts[0]), int(counts[1])
+    verts = np.array([[float(x) for x in t[:3]] for t in lines[pos:pos + nv]], dtype=np.float64).reshape(nv, 3)
+    polygons = []
+    for t in lines[pos + nv:pos + nv + nf]:
+        n = int(t[0])
+        polygons.append([int(x) for x in t[1:1 + n]])
+    return verts.astype(np.float32), _fan(polygons)
+
+
+def read_obj(file_path):
+    """Wavefront OBJ: `v x y z` and `f` lines (indices as i, i/vt, i//vn or i/vt/vn, 1-based or negative = relative to
+    the vertices read so far) -> (vertices [V,3] float32, faces [F,3] int32), polygons fan-triangulated."""
+    verts, polygons = [], []
+    with open(file_path) as fp:
+        for ln in fp:
+            t = ln.split()
+            if not t:
+                continue
+            if t[0] == 'v':
+                verts.append([float(x) for x in t[1:4]])
+            elif t[0] == 'f':
+                idx = [int(x.split('/')[0]) for x in t[1:]]
+                polygons.append([i - 1 if i > 0 else len(verts) + i for i in idx])
+    return np.array(verts, dtype=np.float64).reshape(-1, 3).astype(np.float32), _fan(polygons)
+
+
+def read_stl(file_path):
+    """STL, binary or ASCII -> (vertices [3F,3] float32, faces [F,3] int32): a triangle soup, three vertices per face
+    in file order (the clean stage welds them)."""
+    with open(file_path, 'rb') as fp:
+        data = fp.read()
+    if len(data) >= 84:
+        n = int(np.frombuffer(data[80:84], '<u4')[0])
+        if len(data) == 84 + 50 * n:
+            rec = np.frombuffer(data[84:], dtype=[('n', '<f4', (3,)), ('v', '<f4', (3, 3)), ('attr', '<u2')], count=n)
+            return rec['v'].reshape(-1, 3).copy(), np.arange(3 * n, dtype=np.int32).reshape(-1, 3)
+    text = data.decode('ascii')
+    if not text.lstrip().startswith('solid'):
+        raise ValueError('not an STL file: %s' % file_path)
+    verts = [[float(x) for x in ln.split()[1:4]] for ln in text.split('\n') if ln.strip().startswith('vertex')]
+    if len(verts) % 3:
+        raise ValueError('STL facet without three vertices: %s' % file_path)
+    verts = np.array(verts, dtype=np.float64).reshape(-1, 3).astype(np.float32)
+    return verts, np.arange(len(verts), dtype=np.int32).reshape(-1, 3)
 
 
 def read_mesh(file_path):
-    """Dispatch on the extension (.ply / .off) -> (vertices, faces)."""
+    """Dispatch on the extension (.ply / .off / .obj / .stl) -> (vertices, faces)."""
     ext = os.path.splitext(file_path)[1].lower()
-    if ext == '.ply':
-        return read_ply(file_path)
-    if ext == '.off':
-        return read_off(file_path)
-    raise ValueError('unsupported mesh format: %s' % file_path)
+    readers = {'.ply': read_ply, '.off': read_off, '.obj': read_obj, '.stl': read_stl}
+    if ext not in readers:
+        raise ValueError('unsupported mesh format: %s' % file_path)
+    return readers[ext](file_path)

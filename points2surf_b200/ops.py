@@ -297,6 +297,28 @@ def mesh_signed_distance(verts, faces, query, return_face_ids=False, return_wind
     return out if len(out) > 1 else dist
 
 
+def mesh_clean(verts, faces):
+    """The mesh repair of make_dataset.py:_clean_mesh (rules and output order in include/p2s_b200.h): weld, drop
+    non-finite, degenerate and duplicate faces, fill 3- and 4-edge holes, orient every component consistently and
+    outward when the winding is inconsistent, drop unreferenced vertices.
+    -> (verts [V',3] fp32, faces [F',3] int32, report dict of p2s_clean_report; the four flags as bool)."""
+    verts = _dev(verts, torch.float32, 'verts')
+    faces = _dev(faces, torch.int32, 'faces')
+    if verts.dim() != 2 or verts.shape[1] != 3 or faces.dim() != 2 or faces.shape[1] != 3:
+        raise P2SError('verts and faces must have shape [n, 3]')
+    V, F = verts.shape[0], faces.shape[0]
+    vout = torch.empty((max(V, 1), 3), dtype=torch.float32, device=verts.device)
+    fout = torch.empty((max(2 * F, 1), 3), dtype=torch.int32, device=verts.device)
+    rep = _lib.CleanReport()
+    with torch.cuda.device(verts.device):
+        check(_lib.load().p2s_mesh_clean_dev(_ptr(verts), V, _ptr(faces), F, _ptr(vout), V, _ptr(fout), 2 * F,
+                                             C.byref(rep), _stream()))
+    report = {name: getattr(rep, name) for name, _ in _lib.CleanReport._fields_}
+    for k in ('watertight_before', 'winding_consistent_before', 'watertight', 'winding_consistent'):
+        report[k] = bool(report[k])
+    return vout[:rep.vertices_out], fout[:rep.faces_out], report
+
+
 SCANNER_DEFAULTS = dict(res_x=176, res_y=144, lens_angle_w=43.6, lens_angle_h=34.6, max_distance=10.0, noise_mu=0.0)
 
 
