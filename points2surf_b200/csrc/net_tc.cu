@@ -441,6 +441,12 @@ __global__ void guard_scatter_kernel(const float* __restrict__ src, const int32_
     logits[(int64_t)list[i] * 2 + 0] = src[i * 2 + 0];
     logits[(int64_t)list[i] * 2 + 1] = src[i * 2 + 1];
 }
+__global__ void guard_scatter_rows_kernel(const float* __restrict__ src, const int32_t* __restrict__ list, int n, int row_floats, float* __restrict__ dst) {
+    int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= (int64_t)n * row_floats) return;
+    int i = (int)(e / row_floats), j = (int)(e % row_floats);
+    dst[(int64_t)list[i] * row_floats + j] = src[e];
+}
 
 }  // namespace
 
@@ -829,13 +835,26 @@ void forward_tc(Model& m, const float* patch, const float* sub, const float* que
         m.last_guard_count += n;
         if (n > 0) {
             const size_t rowp = (size_t)P * 3, rows = (size_t)S * 3;
-            float* gbuf = m.ws_misc.as<float>((size_t)n * (rowp + rows + 3 + 2) + 64);
+            float* const aux = m.debug_aux;
+            const size_t aux_floats = aux ? (size_t)n * kAuxStride : 0;
+            float* gbuf = m.ws_misc.as<float>((size_t)n * (rowp + rows + 3 + 2) + 64 + aux_floats);
             float* gp = gbuf; float* gs = gp + (size_t)n * rowp; float* gq = gs + (size_t)n * rows; float* gl = gq + ((size_t)n * 3 + 3) / 4 * 4;
+            float* gaux = gl + ((size_t)n * 2 + 3) / 4 * 4;
             P2S_LAUNCH(guard_gather_kernel, (unsigned)cdiv((int64_t)n * rowp, 256), 256, 0, st, patch, list, n, (int)rowp, gp);
             P2S_LAUNCH(guard_gather_kernel, (unsigned)cdiv((int64_t)n * rows, 256), 256, 0, st, sub, list, n, (int)rows, gs);
             P2S_LAUNCH(guard_gather_kernel, (unsigned)cdiv((int64_t)n * 3, 256), 256, 0, st, query, list, n, 3, gq);
-            forward_guard(m, gp, gs, gq, n, gl, st);
+            // the recompute sees the flagged queries in list order: its diagnostics go to scratch rows and are scattered
+            // back to the queries' own rows, like the logits
+            if (aux) m.debug_aux = gaux;
+            try {
+                forward_guard(m, gp, gs, gq, n, gl, st);
+            } catch (...) {
+                m.debug_aux = aux;
+                throw;
+            }
+            m.debug_aux = aux;
             P2S_LAUNCH(guard_scatter_kernel, (unsigned)cdiv(n, 256), 256, 0, st, gl, list, n, logits);
+            if (aux) P2S_LAUNCH(guard_scatter_rows_kernel, (unsigned)cdiv((int64_t)n * kAuxStride, 256), 256, 0, st, gaux, list, n, (int)kAuxStride, aux);
         }
     }
 }
