@@ -226,6 +226,21 @@ int p2s_chamfer_hausdorff_dev(const float* a, int64_t na, const float* b, int64_
 int p2s_mesh_signed_distance_dev(const float* verts, int64_t V, const int32_t* faces, int64_t F, const float* query,
                                  int64_t Q, float* dist, int32_t* closest_face, float* winding, void* stream);
 
+/* The unsigned point-to-mesh query: trimesh.proximity.closest_point as called by point_cloud.get_closest_distance_batched
+ * (source/base/point_cloud.py:195-218; source/figure/distance_vis.py, and the ground-truth normals of eval_dataset.py).
+ * The distance and the face come from the same pass as p2s_mesh_signed_distance_dev without the solid angles: the same
+ * fp32 prefilter and float64 recompute band, the same face slabs and the same tie rule (lowest face index), so dist and
+ * closest_face equal that function's |dist| and closest_face bit for bit.  The closest point is computed in float64 on
+ * the winning face, by the rule that gave its distance: the orthogonal projection onto the face's plane when the query
+ * projects inside the face, else the closest point of the nearest edge (the first of ab, bc, ca on equal distances;
+ * zero-area faces are their edges), then rounded to fp32 once.  A query with a non-finite coordinate gives NaN for the
+ * distance and the point, and face -1.
+ *   verts [V,3] fp32, faces [F,3] int32 (every index in [0, V), else an error; F > 0), query [Q,3] fp32
+ *   closest_pts [Q,3] fp32 or NULL; dist [Q] fp32; closest_face [Q] int32 or NULL.
+ * Bitwise deterministic, independent of how the queries are split across calls.  sync: index check read-back. */
+int p2s_mesh_closest_point_dev(const float* verts, int64_t V, const int32_t* faces, int64_t F, const float* query,
+                               int64_t Q, float* closest_pts, float* dist, int32_t* closest_face, void* stream);
+
 /* ------------------------------------------------------------------ input point clouds --------- */
 /* Simulated time-of-flight range scans: the BlenSor scans of make_dataset.py:sample_blensor (make_dataset.py:242-380,
  * scanner settings blensor_script_template.py:80-96) merged in model space like _pcd_files_to_pts

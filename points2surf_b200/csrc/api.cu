@@ -471,6 +471,14 @@ int p2s_mesh_signed_distance_dev(const float* verts, int64_t V, const int32_t* f
     });
 }
 
+int p2s_mesh_closest_point_dev(const float* verts, int64_t V, const int32_t* faces, int64_t F, const float* query,
+                               int64_t Q, float* closest_pts, float* dist, int32_t* closest_face, void* stream) {
+    return guarded([&] {
+        P2S_CHECK(verts && faces && ((query && dist) || Q == 0), "null argument");
+        mesh_closest_point(verts, V, faces, F, query, Q, closest_pts, dist, closest_face, as_stream(stream));
+    });
+}
+
 int p2s_range_scan_dev(const float* verts, int64_t V, const int32_t* faces, int64_t F, const double* poses, int64_t S,
                        const p2s_scan_config* cfg, uint64_t seed, float* pts_noisy, float* pts_clean, int32_t* face_ids,
                        int64_t cap, int32_t* hits_per_scan, int64_t* total_host, void* stream) {

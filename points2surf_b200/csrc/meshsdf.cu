@@ -14,6 +14,11 @@
 //   3. meshsdf_finalize_kernel: slabs in ascending order (min d^2, strict <; winding sum) -> signed distance.
 // No float atomics anywhere: results are bitwise identical across runs and for any split of the query array.
 //
+// The unsigned query (p2s_mesh_closest_point_dev: trimesh.proximity.closest_point for point_cloud.
+// get_closest_distance_batched, source/base/point_cloud.py:195-218) is the same slab kernel compiled without the solid
+// angles (meshsdf_slab_kernel<false>), so its distances and faces are the signed path's bit for bit; its finalize
+// recomputes the closest point of the winning face in float64 (tri_dist2 with a point output) and rounds it once.
+//
 // Sign: inside iff the generalised winding number w (Jacobson et al. 2013) > 0.5, inside is positive like trimesh;
 // |d| <= 1e-8 counts as on the surface and is positive (trimesh's tol.merge).  On a closed, consistently oriented mesh
 // w is 1 inside and 0 outside.  On a mesh with holes or inconsistent orientation w is fractional and can disagree with
@@ -41,23 +46,27 @@ constexpr float kEpsScale = 1.0f / 4096.0f;
 
 enum : unsigned char { kZeroArea = 1, kForce64 = 2 };
 
-// squared distance from p to the segment [a, b] (a point when a == b)
+// squared distance from p to the segment [a, b] (a point when a == b); the closest point a + t (b - a) into cp when
+// cp is not null
 template <class T>
-__device__ __forceinline__ T seg_dist2(T px, T py, T pz, T ax, T ay, T az, T bx, T by, T bz) {
+__device__ __forceinline__ T seg_dist2(T px, T py, T pz, T ax, T ay, T az, T bx, T by, T bz, T* cp = nullptr) {
     const T ux = bx - ax, uy = by - ay, uz = bz - az;
     const T wx = px - ax, wy = py - ay, wz = pz - az;
     const T uu = ux * ux + uy * uy + uz * uz;
     T t = uu > T(0) ? (ux * wx + uy * wy + uz * wz) / uu : T(0);
     t = t < T(0) ? T(0) : (t > T(1) ? T(1) : t);
     const T dx = wx - t * ux, dy = wy - t * uy, dz = wz - t * uz;
+    if (cp) { cp[0] = ax + t * ux; cp[1] = ay + t * uy; cp[2] = az + t * uz; }
     return dx * dx + dy * dy + dz * dz;
 }
 
 // squared distance from p to the triangle (a, b, c): the plane distance when p projects inside the triangle, else the
-// nearest edge.  A zero-area face is its three edges (a segment or a point).
+// nearest edge.  A zero-area face is its three edges (a segment or a point).  When cp is not null, the point that gives
+// this distance goes to cp: the projection onto the plane, or the closest point of the first nearest edge in the order
+// ab, bc, ca.  With cp null the arithmetic is exactly the distance-only one.
 template <class T>
 __device__ __forceinline__ T tri_dist2(T px, T py, T pz, T ax, T ay, T az, T bx, T by, T bz, T cx, T cy, T cz,
-                                       bool zero_area) {
+                                       bool zero_area, T* cp = nullptr) {
     if (!zero_area) {
         const T abx = bx - ax, aby = by - ay, abz = bz - az;
         const T acx = cx - ax, acy = cy - ay, acz = cz - az;
@@ -74,12 +83,50 @@ __device__ __forceinline__ T tri_dist2(T px, T py, T pz, T ax, T ay, T az, T bx,
         const T e2 = (cay * cpz - caz * cpy) * nx + (caz * cpx - cax * cpz) * ny + (cax * cpy - cay * cpx) * nz;
         if (nn > T(0) && e0 >= T(0) && e1 >= T(0) && e2 >= T(0)) {
             const T h = nx * apx + ny * apy + nz * apz;
+            if (cp) {
+                const T s = h / nn;
+                cp[0] = px - s * nx; cp[1] = py - s * ny; cp[2] = pz - s * nz;
+            }
             return h * h / nn;
         }
     }
-    T d = seg_dist2(px, py, pz, ax, ay, az, bx, by, bz);
-    d = fmin(d, seg_dist2(px, py, pz, bx, by, bz, cx, cy, cz));
-    return fmin(d, seg_dist2(px, py, pz, cx, cy, cz, ax, ay, az));
+    if (!cp) {
+        T d = seg_dist2(px, py, pz, ax, ay, az, bx, by, bz);
+        d = fmin(d, seg_dist2(px, py, pz, bx, by, bz, cx, cy, cz));
+        return fmin(d, seg_dist2(px, py, pz, cx, cy, cz, ax, ay, az));
+    }
+    T e[3];
+    T d = seg_dist2(px, py, pz, ax, ay, az, bx, by, bz, cp);
+    const T d1 = seg_dist2(px, py, pz, bx, by, bz, cx, cy, cz, e);
+    if (d1 < d) { d = d1; cp[0] = e[0]; cp[1] = e[1]; cp[2] = e[2]; }
+    const T d2 = seg_dist2(px, py, pz, cx, cy, cz, ax, ay, az, e);
+    if (d2 < d) { d = d2; cp[0] = e[0]; cp[1] = e[1]; cp[2] = e[2]; }
+    return d;
+}
+
+// kZeroArea / kForce64 of the face with corners c = (a, b, c)
+__device__ __forceinline__ unsigned char face_flags(const float* c) {
+    // zero area: the float64 cross product of the edges is exactly 0 (no FMA contraction, so that the CPU restatement
+    // makes the same decision)
+    const double ux = (double)c[3] - c[0], uy = (double)c[4] - c[1], uz = (double)c[5] - c[2];
+    const double wx = (double)c[6] - c[0], wy = (double)c[7] - c[1], wz = (double)c[8] - c[2];
+    const double nx = __dsub_rn(__dmul_rn(uy, wz), __dmul_rn(uz, wy));
+    const double ny = __dsub_rn(__dmul_rn(uz, wx), __dmul_rn(ux, wz));
+    const double nz = __dsub_rn(__dmul_rn(ux, wy), __dmul_rn(uy, wx));
+    const double nn = nx * nx + ny * ny + nz * nz;
+    const double vx = (double)c[6] - c[3], vy = (double)c[7] - c[4], vz = (double)c[8] - c[5];
+    const double l2 = fmax(ux * ux + uy * uy + uz * uz, fmax(wx * wx + wy * wy + wz * wz, vx * vx + vy * vy + vz * vz));
+    const bool zero = nx == 0.0 && ny == 0.0 && nz == 0.0;
+    return zero ? (kZeroArea | kForce64) : (nn < (1.0 / 1024.0) * l2 * l2 ? kForce64 : 0);
+}
+
+__device__ __forceinline__ void load_face(const float* __restrict__ verts, const int32_t* __restrict__ faces, int64_t f,
+                                          float* c) {
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+        const int64_t vi = faces[3 * f + k];
+        c[3 * k] = verts[3 * vi]; c[3 * k + 1] = verts[3 * vi + 1]; c[3 * k + 2] = verts[3 * vi + 2];
+    }
 }
 
 __global__ void __launch_bounds__(256)
@@ -101,7 +148,9 @@ mesh_check_kernel(const float* __restrict__ verts, int64_t V, const int32_t* __r
     }
 }
 
-// grid (ceil(Q / kThreads), slabs): slab s covers faces [s * slab_len, min(F, (s + 1) * slab_len))
+// grid (ceil(Q / kThreads), slabs): slab s covers faces [s * slab_len, min(F, (s + 1) * slab_len)).
+// kWinding = false is the unsigned query: the same distances and faces, no solid angles, part_wind unused.
+template <bool kWinding>
 __global__ void __launch_bounds__(kThreads)
 meshsdf_slab_kernel(const float* __restrict__ verts, const int32_t* __restrict__ faces, int64_t F, int64_t slab_len,
                     const float* __restrict__ query, int64_t Q, float vmax, double* __restrict__ part_d2,
@@ -121,27 +170,11 @@ meshsdf_slab_kernel(const float* __restrict__ verts, const int32_t* __restrict__
         const int cnt = (int)min((int64_t)kTile, f1 - t);
         __syncthreads();
         if (threadIdx.x < cnt) {
-            const int64_t f = t + threadIdx.x;
             float c[9];
-#pragma unroll
-            for (int k = 0; k < 3; ++k) {
-                const int64_t vi = faces[3 * f + k];
-                c[3 * k] = verts[3 * vi]; c[3 * k + 1] = verts[3 * vi + 1]; c[3 * k + 2] = verts[3 * vi + 2];
-            }
+            load_face(verts, faces, t + threadIdx.x, c);
 #pragma unroll
             for (int k = 0; k < 9; ++k) sv[k][threadIdx.x] = c[k];
-            // zero area: the float64 cross product of the edges is exactly 0 (no FMA contraction, so that the CPU
-            // restatement makes the same decision)
-            const double ux = (double)c[3] - c[0], uy = (double)c[4] - c[1], uz = (double)c[5] - c[2];
-            const double wx = (double)c[6] - c[0], wy = (double)c[7] - c[1], wz = (double)c[8] - c[2];
-            const double nx = __dsub_rn(__dmul_rn(uy, wz), __dmul_rn(uz, wy));
-            const double ny = __dsub_rn(__dmul_rn(uz, wx), __dmul_rn(ux, wz));
-            const double nz = __dsub_rn(__dmul_rn(ux, wy), __dmul_rn(uy, wx));
-            const double nn = nx * nx + ny * ny + nz * nz;
-            const double vx = (double)c[6] - c[3], vy = (double)c[7] - c[4], vz = (double)c[8] - c[5];
-            const double l2 = fmax(ux * ux + uy * uy + uz * uz, fmax(wx * wx + wy * wy + wz * wz, vx * vx + vy * vy + vz * vz));
-            const bool zero = nx == 0.0 && ny == 0.0 && nz == 0.0;
-            sflag[threadIdx.x] = zero ? (kZeroArea | kForce64) : (nn < (1.0 / 1024.0) * l2 * l2 ? kForce64 : 0);
+            sflag[threadIdx.x] = face_flags(c);
         }
         __syncthreads();
         if (i >= Q) continue;
@@ -163,7 +196,7 @@ meshsdf_slab_kernel(const float* __restrict__ verts, const int32_t* __restrict__
                     thr = best32 + kRelTol * best32 + 2.f * sqrtf(best32) * eps + eps * eps;
                 }
             }
-            if (!zero) {
+            if (kWinding && !zero) {
                 const double Ax = ax - qx, Ay = ay - qy, Az = az - qz;
                 const double Bx = bx - qx, By = by - qy, Bz = bz - qz;
                 const double Cx = cx - qx, Cy = cy - qy, Cz = cz - qz;
@@ -181,7 +214,7 @@ meshsdf_slab_kernel(const float* __restrict__ verts, const int32_t* __restrict__
         const int64_t o = (int64_t)blockIdx.y * Q + i;
         part_d2[o] = best64;
         part_face[o] = best_face;
-        part_wind[o] = wind;
+        if (kWinding) part_wind[o] = wind;
     }
 }
 
@@ -208,6 +241,34 @@ meshsdf_finalize_kernel(const double* __restrict__ part_d2, const int32_t* __res
     if (winding) winding[i] = (float)w;
 }
 
+// slabs in ascending order (min d^2, strict <) -> unsigned distance, face, and the closest point: tri_dist2's point on
+// the winning face in float64, rounded to fp32 once
+__global__ void __launch_bounds__(256)
+mesh_closest_finalize_kernel(const double* __restrict__ part_d2, const int32_t* __restrict__ part_face, int slabs,
+                             int64_t Q, const float* __restrict__ verts, const int32_t* __restrict__ faces,
+                             const float* __restrict__ query, float* __restrict__ closest, float* __restrict__ dist,
+                             int32_t* __restrict__ closest_face) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= Q) return;
+    double bd = INFINITY;
+    int32_t bf = -1;
+    for (int s = 0; s < slabs; ++s) {
+        const double d = part_d2[(int64_t)s * Q + i];
+        if (d < bd) { bd = d; bf = part_face[(int64_t)s * Q + i]; }   // strict <: the lower slab (lower face) wins ties
+    }
+    dist[i] = bf < 0 ? NAN : (float)sqrt(bd);   // bf < 0: a non-finite query coordinate
+    if (closest_face) closest_face[i] = bf;
+    if (!closest) return;
+    double cp[3] = {NAN, NAN, NAN};
+    if (bf >= 0) {
+        float c[9];
+        load_face(verts, faces, bf, c);
+        tri_dist2<double>(query[3 * i], query[3 * i + 1], query[3 * i + 2], c[0], c[1], c[2], c[3], c[4], c[5], c[6], c[7],
+                          c[8], face_flags(c) & kZeroArea, cp);
+    }
+    closest[3 * i] = (float)cp[0]; closest[3 * i + 1] = (float)cp[1]; closest[3 * i + 2] = (float)cp[2];
+}
+
 struct Scratch {
     DevBuf flags, d2, face, wind;
 };
@@ -216,10 +277,10 @@ Scratch& scratch() {
     return s;
 }
 
-}  // namespace
-
-void mesh_signed_distance(const float* verts, int64_t V, const int32_t* faces, int64_t F, const float* query, int64_t Q,
-                          float* dist, int32_t* closest_face, float* winding, cudaStream_t st) {
+// kSigned: signed distance (+ winding); else unsigned distance (+ closest point)
+template <bool kSigned>
+void mesh_query(const float* verts, int64_t V, const int32_t* faces, int64_t F, const float* query, int64_t Q,
+                float* dist, int32_t* closest_face, float* winding, float* closest, cudaStream_t st) {
     P2S_CHECK(V > 0 && F > 0, "empty mesh");
     P2S_CHECK(V <= INT32_MAX && F <= INT32_MAX / 3, "mesh too large for int32 indices");
     auto& sc = scratch();
@@ -241,14 +302,31 @@ void mesh_signed_distance(const float* verts, int64_t V, const int32_t* faces, i
     const int64_t qc = std::min(Q, kChunk);
     double* d2 = sc.d2.as<double>((size_t)slabs * qc);
     int32_t* fc = sc.face.as<int32_t>((size_t)slabs * qc);
-    double* wn = sc.wind.as<double>((size_t)slabs * qc);
+    double* wn = kSigned ? sc.wind.as<double>((size_t)slabs * qc) : nullptr;
     for (int64_t q0 = 0; q0 < Q; q0 += kChunk) {
         const int64_t nq = std::min(kChunk, Q - q0);
-        P2S_LAUNCH(meshsdf_slab_kernel, dim3((unsigned)cdiv(nq, kThreads), (unsigned)slabs), kThreads, 0, st, verts, faces,
-                   F, slab_len, query + 3 * q0, nq, vmax, d2, fc, wn);
-        P2S_LAUNCH(meshsdf_finalize_kernel, (unsigned)cdiv(nq, 256), 256, 0, st, d2, fc, wn, slabs, nq, dist + q0,
-                   closest_face ? closest_face + q0 : nullptr, winding ? winding + q0 : nullptr);
+        P2S_LAUNCH(meshsdf_slab_kernel<kSigned>, dim3((unsigned)cdiv(nq, kThreads), (unsigned)slabs), kThreads, 0, st, verts,
+                   faces, F, slab_len, query + 3 * q0, nq, vmax, d2, fc, wn);
+        if (kSigned)
+            P2S_LAUNCH(meshsdf_finalize_kernel, (unsigned)cdiv(nq, 256), 256, 0, st, d2, fc, wn, slabs, nq, dist + q0,
+                       closest_face ? closest_face + q0 : nullptr, winding ? winding + q0 : nullptr);
+        else
+            P2S_LAUNCH(mesh_closest_finalize_kernel, (unsigned)cdiv(nq, 256), 256, 0, st, d2, fc, slabs, nq, verts, faces,
+                       query + 3 * q0, closest ? closest + 3 * q0 : nullptr, dist + q0,
+                       closest_face ? closest_face + q0 : nullptr);
     }
+}
+
+}  // namespace
+
+void mesh_signed_distance(const float* verts, int64_t V, const int32_t* faces, int64_t F, const float* query, int64_t Q,
+                          float* dist, int32_t* closest_face, float* winding, cudaStream_t st) {
+    mesh_query<true>(verts, V, faces, F, query, Q, dist, closest_face, winding, nullptr, st);
+}
+
+void mesh_closest_point(const float* verts, int64_t V, const int32_t* faces, int64_t F, const float* query, int64_t Q,
+                        float* closest, float* dist, int32_t* closest_face, cudaStream_t st) {
+    mesh_query<false>(verts, V, faces, F, query, Q, dist, closest_face, nullptr, closest, st);
 }
 
 }  // namespace p2s

@@ -297,6 +297,25 @@ def mesh_signed_distance(verts, faces, query, return_face_ids=False, return_wind
     return out if len(out) > 1 else dist
 
 
+def mesh_closest_point(verts, faces, query):
+    """Closest point on the mesh of every query point (trimesh.proximity.closest_point, as called by
+    source/base/point_cloud.py:195-218) -> (closest [Q,3] fp32, unsigned distance [Q] fp32, face [Q] int32, lowest index
+    on ties).  Distance and face equal mesh_signed_distance's |d| and face bit for bit; rules in include/p2s_b200.h."""
+    verts = _dev(verts, torch.float32, 'verts')
+    faces = _dev(faces, torch.int32, 'faces')
+    q = _dev(query, torch.float32, 'query')
+    if verts.dim() != 2 or verts.shape[1] != 3 or faces.dim() != 2 or faces.shape[1] != 3 or q.dim() != 2 or q.shape[1] != 3:
+        raise P2SError('verts, faces and query must have shape [n, 3]')
+    Q = q.shape[0]
+    closest = torch.empty((Q, 3), dtype=torch.float32, device=q.device)
+    dist = torch.empty((Q,), dtype=torch.float32, device=q.device)
+    fid = torch.empty((Q,), dtype=torch.int32, device=q.device)
+    with torch.cuda.device(q.device):
+        check(_lib.load().p2s_mesh_closest_point_dev(_ptr(verts), verts.shape[0], _ptr(faces), faces.shape[0], _ptr(q), Q,
+                                                     _ptr(closest), _ptr(dist), _ptr(fid), _stream()))
+    return closest, dist, fid
+
+
 def mesh_clean(verts, faces):
     """The mesh repair of make_dataset.py:_clean_mesh (rules and output order in include/p2s_b200.h): weld, drop
     non-finite, degenerate and duplicate faces, fill 3- and 4-edge holes, orient every component consistently and

@@ -36,6 +36,18 @@ def torus_mesh(dev, min_faces=45000):
     raise RuntimeError('no torus mesh with %d faces' % min_faces)
 
 
+def torus_queries(v, f, rng, n=150000):
+    """n queries, half within the patch radius 6/256 of the surface, half uniform in [-0.5, 0.5)^3"""
+    n_near = n // 2
+    fi = rng.choice(len(f), n_near)
+    r = rng.uniform(0, 1, (n_near, 2))
+    r[r.sum(1) > 1] = 1 - r[r.sum(1) > 1]
+    va, vb, vc = v[f[fi, 0]], v[f[fi, 1]], v[f[fi, 2]]
+    near = va + r[:, :1] * (vb - va) + r[:, 1:] * (vc - va) + rng.uniform(-6 / 256, 6 / 256, (n_near, 1)) * \
+        np.cross(vb - va, vc - va) / (np.linalg.norm(np.cross(vb - va, vc - va), axis=1, keepdims=True) + 1e-30)
+    return np.concatenate([near, rng.uniform(-0.5, 0.5, (n - n_near, 3))]).astype(np.float32)
+
+
 def time_calls(calls, reps):
     for c in calls:
         c()
@@ -67,14 +79,7 @@ def main():
 
     v, f, res = torus_mesh(dev)
     rng = np.random.RandomState(0)
-    n_near = 75000
-    fi = rng.choice(len(f), n_near)
-    r = rng.uniform(0, 1, (n_near, 2))
-    r[r.sum(1) > 1] = 1 - r[r.sum(1) > 1]
-    va, vb, vc = v[f[fi, 0]], v[f[fi, 1]], v[f[fi, 2]]
-    near = va + r[:, :1] * (vb - va) + r[:, 1:] * (vc - va) + rng.uniform(-6 / 256, 6 / 256, (n_near, 1)) * \
-        np.cross(vb - va, vc - va) / (np.linalg.norm(np.cross(vb - va, vc - va), axis=1, keepdims=True) + 1e-30)
-    q = np.concatenate([near, rng.uniform(-0.5, 0.5, (150000 - n_near, 3))]).astype(np.float32)
+    q = torus_queries(v, f, rng)
     vt, ft, qt = torch.from_numpy(v).to(dev), torch.from_numpy(f).to(dev), torch.from_numpy(q).to(dev)
     big_ms = time_calls([lambda: ops.mesh_signed_distance(vt, ft, qt)], a.reps)
 
