@@ -320,6 +320,54 @@ typedef struct {
 int p2s_mesh_clean_dev(const float* verts, int64_t V, const int32_t* faces, int64_t F, float* verts_out, int64_t vcap,
                        int32_t* faces_out, int64_t fcap, p2s_clean_report* report_host, void* stream);
 
+/* ------------------------------------------------------------------ screened Poisson baseline --- */
+/* Screened Poisson surface reconstruction from oriented points, the SPSR baseline of eval_dataset.py:142-158 (which
+ * the reference runs through meshlabserver with poisson.mlx).  The discrete system:
+ *   domain  the cube of edge E = scale * (largest extent of the bounding box of all N points), centred on that box,
+ *           mapped to [0,1]^3; nodes k in [0, 2^depth]^3, spacing h = 2^-depth
+ *   basis   trilinear hat functions B_k, all nodes free (natural boundary); chi is trilinear in every cell
+ *   1D      M = int phi_i phi_j (2h/3 on the diagonal, h/3 at both ends, h/6 off it), K = int phi_i' phi_j' (2/h, 1/h at
+ *           the ends, -1/h), D(i, j) = int phi_i phi_j' (+-1/2 off the diagonal; -1/2 at node 0, +1/2 at node 2^depth)
+ *   L       K(x)M(x)M + M(x)K(x)M + M(x)M(x)K (the 27-point Q1 stencil)
+ *   points  normals scaled to unit length; a zero normal drops the point (counted).  Area weight a_p = (4h)^2 / n_c(p),
+ *           n_c = the number of kept points in p's cell at depth - 2
+ *   V       V_k = sum_p a_p n_p B_k(p) / h^3;  b_j = int V . grad B_j
+ *   S       alpha sum_p a_p B(p) B(p)^T, alpha = point_weight * 2^depth
+ *   solve   (L + S) chi = b by conjugate gradients preconditioned with one symmetric multigrid V-cycle over depths
+ *           depth..2 (exact Galerkin levels, `iters` damped-Jacobi sweeps before and after each coarse correction, 128
+ *           sweeps on depth 2); stop at ||b - A chi|| / ||b|| <= 1e-5, after 100 iterations, or when the residual has
+ *           not reached a new minimum for 10 iterations
+ *   iso     sum a_p chi(p) / sum a_p
+ * values [(2^depth+1)^3] fp32 = iso - chi at node (i, j, k), index (i R + j) R + k with R = 2^depth + 1: positive inside,
+ * zero on the surface, so p2s_marching_cubes_dev(values, R, 0) extracts it; node (i, j, k) is at world position
+ * origin + edge (i, j, k) / 2^depth.  values == NULL with vcap == 0 only validates the config and sets grid_res.
+ * Deviations from PoissonRecon: a dense grid instead of an adaptive octree (samplesPerNode, fullDepth unused), degree-1
+ * instead of degree-2 B-splines, no confidence, and the scaling of alpha is unpinned (PoissonRecon's is not
+ * available to compare against).  Errors (not faults): N = 0, non-finite points or normals, zero extent, every normal
+ * zero, depth outside [2, 9], scale < 1, point_weight < 0, iters outside [1, 64].
+ * Bitwise deterministic (fixed-order sums, no float atomics).  sync: several read-backs (sizes, CG residuals). */
+typedef struct {
+    int32_t depth;          /* 8 in poisson.mlx */
+    float point_weight;     /* 4 */
+    float scale;            /* 1.1 */
+    int32_t iters;          /* 8: smoothing sweeps per level and half V-cycle */
+} p2s_poisson_config;
+
+typedef struct {
+    double origin[3];       /* world position of node (0, 0, 0) */
+    double edge;            /* world edge of the cube */
+    double iso;             /* iso-value of chi (values = iso - chi) */
+    double residual;        /* ||b - A chi|| / ||b|| at exit; 0 when b = 0 */
+    int64_t grid_res;       /* 2^depth + 1 nodes per axis */
+    int64_t points_used, dropped_points;
+    int64_t occupied_cells; /* finest cells holding at least one kept point */
+    int32_t iterations, reserved;
+    float stage_ms[4];      /* CUDA-event times of setup (sort, cells, levels), right-hand side, solve, iso + output */
+} p2s_poisson_report;
+
+int p2s_poisson_solve_dev(const float* pts, const float* normals, int64_t N, const p2s_poisson_config* cfg, float* values,
+                          int64_t vcap, p2s_poisson_report* report_host, void* stream);
+
 /* ------------------------------------------------------------------ training-step primitives --- */
 /* Row a14 (SURVEY.md section 8a): loss + backward + SGD of source/points_to_surf_train.py:441-461,537-563 with the
  * train-mode BatchNorm of source/points_to_surf_model.py.  Activations are row-major [rows, C] fp32.  The host side

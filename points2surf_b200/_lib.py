@@ -34,6 +34,17 @@ class CleanReport(C.Structure):
         [('volume', C.c_double)]
 
 
+class PoissonConfig(C.Structure):
+    _fields_ = [('depth', C.c_int32), ('point_weight', C.c_float), ('scale', C.c_float), ('iters', C.c_int32)]
+
+
+class PoissonReport(C.Structure):
+    _fields_ = [('origin', C.c_double * 3), ('edge', C.c_double), ('iso', C.c_double), ('residual', C.c_double),
+                ('grid_res', C.c_int64), ('points_used', C.c_int64), ('dropped_points', C.c_int64),
+                ('occupied_cells', C.c_int64), ('iterations', C.c_int32), ('reserved', C.c_int32),
+                ('stage_ms', C.c_float * 4)]
+
+
 PRECISION_FP32, PRECISION_TC = 0, 1
 SUBSAMPLE_WEIGHTED, SUBSAMPLE_UNIFORM = 0, 1
 
@@ -93,6 +104,8 @@ SIGNATURES = {
     'p2s_range_scan_dev': (C.c_int, [_vp, _i64, _vp, _i64, _vp, _i64, C.POINTER(ScanConfig), C.c_uint64, _vp, _vp, _vp,
                                      _i64, _vp, C.POINTER(_i64), _vp]),
     'p2s_mesh_clean_dev': (C.c_int, [_vp, _i64, _vp, _i64, _vp, _i64, _vp, _i64, C.POINTER(CleanReport), _vp]),
+    'p2s_poisson_solve_dev': (C.c_int, [_vp, _vp, _i64, C.POINTER(PoissonConfig), _vp, _i64, C.POINTER(PoissonReport),
+                                        _vp]),
 }
 
 _lib = None

@@ -497,6 +497,14 @@ int p2s_mesh_clean_dev(const float* verts, int64_t V, const int32_t* faces, int6
     });
 }
 
+int p2s_poisson_solve_dev(const float* pts, const float* normals, int64_t N, const p2s_poisson_config* cfg, float* values,
+                          int64_t vcap, p2s_poisson_report* report_host, void* stream) {
+    return guarded([&] {
+        P2S_CHECK(cfg && report_host, "null argument");
+        poisson_solve(pts, normals, N, *cfg, values, vcap, report_host, as_stream(stream));
+    });
+}
+
 // ---- training-step primitives (train_ops.cu)
 #define P2S_OP(name, params, ...)                                   \
     int name params { return guarded([&] { __VA_ARGS__; }); }

@@ -126,6 +126,9 @@ void range_scan(const float* verts, int64_t V, const int32_t* faces, int64_t F, 
 // meshclean.cu
 void mesh_clean(const float* verts, int64_t V, const int32_t* faces, int64_t F, float* verts_out, int64_t vcap,
                 int32_t* faces_out, int64_t fcap, p2s_clean_report* report, cudaStream_t st);
+// poisson.cu
+void poisson_solve(const float* pts, const float* normals, int64_t N, const p2s_poisson_config& cfg, float* values,
+                   int64_t cap, p2s_poisson_report* report, cudaStream_t st);
 // gemm_tn_tc.cu
 bool gemm_tn_tc_ok(const float* A, int lda, const float* B, int ldb, int64_t M, int N, int K);
 void launch_gemm_tn_tc(const float* A, int lda, const float* B, int ldb, float* C, int ldc, int64_t M, int N, int K,

@@ -7,19 +7,33 @@ which the "SPSR + GT normals" baseline reconstructs from, with the point-to-mesh
 
 writes DATASET_DIR/06_normals/<name>.xyz.npy and 06_normals/pts/<name>.xyz from 04_pts and 03_meshes with 100 000 samples
 per mesh, like eval_dataset.py:143-146.  The Screened-Poisson stages of eval_dataset.py need meshlabserver and are not
-run."""
+run; with --spsr
+
+    python -m points2surf_b200.eval_dataset DATASET_DIR --spsr
+
+the "SPSR + GT normals" stage of eval_dataset.py:143-158 runs instead, with the reconstruction on the GPU
+(apply_meshlab_filter, points2surf_b200/poisson.py): 06_normals, then 06_poisson_rec_gt_normals/<name>.ply, then
+comp_poisson_rec_gt_normals.csv against 03_meshes for the shapes in valset.txt."""
 import argparse
 import os
 import sys
+import xml.etree.ElementTree as ET
 
 import numpy as np
 import torch
 
+from . import evaluation
 from . import make_dataset
 from . import mesh_io
 from . import ops
 from . import point_cloud
+from . import poisson
 from . import sdf
+
+# the Screened Poisson parameters of the reference's poisson.mlx that this reconstruction uses
+POISSON_MLX_DEFAULTS = dict(depth=8, point_weight=4.0, scale=1.1, iters=8)
+_MLX_PARAMS = dict(depth=('depth', int), pointWeight=('point_weight', float), scale=('scale', float),
+                   iters=('iters', int))
 
 
 def _face_normals_dev(verts, faces):
@@ -83,17 +97,76 @@ def get_pts_normals(base_dir, dataset_dir, dir_in_pointcloud, dir_in_meshes, dir
             _get_pts_normals_single_file(pts_in, mesh_in, normals_out, pts_normals_out, samples_per_model)
 
 
+def read_poisson_filter(filter_file):
+    """depth / point_weight / scale / iters of the Screened Poisson filter in a meshlab filter script (.mlx), the
+    poisson.mlx defaults for a parameter it does not set.  Raises ValueError when the script holds any other filter."""
+    params = dict(POISSON_MLX_DEFAULTS)
+    filters = [e for e in ET.parse(filter_file).getroot() if e.tag in ('filter', 'xmlfilter')]
+    names = [e.get('name', '') for e in filters]
+    if len(filters) != 1 or 'screened poisson' not in names[0].lower():
+        raise ValueError('{}: only a single Screened Poisson filter is supported, found {}'.format(filter_file, names))
+    for p in filters[0]:
+        if p.get('name') in _MLX_PARAMS:
+            key, conv = _MLX_PARAMS[p.get('name')]
+            params[key] = conv(p.get('value'))
+    return params
+
+
+def apply_meshlab_filter(base_dir, dataset_dir, pts_dir, recon_mesh_dir, num_processes, filter_file, meshlabserver_bin):
+    """eval_dataset.py:50-67 without meshlab: Screened Poisson reconstruction (points2surf_b200/poisson.py) of every
+    <pts_dir>/<name>.xyz (text x y z nx ny nz, as point_cloud.write_xyz writes it) into <recon_mesh_dir>/<name>.ply,
+    unless that is newer than its input.  The parameters come from `filter_file` when it exists (read_poisson_filter),
+    else from poisson.mlx (POISSON_MLX_DEFAULTS).  `num_processes` and `meshlabserver_bin` are accepted and ignored."""
+    params = read_poisson_filter(filter_file) if filter_file and os.path.isfile(filter_file) \
+        else dict(POISSON_MLX_DEFAULTS)
+    pts_dir_abs = os.path.join(base_dir, dataset_dir, pts_dir)
+    recon_mesh_dir_abs = os.path.join(base_dir, dataset_dir, recon_mesh_dir)
+    os.makedirs(recon_mesh_dir_abs, exist_ok=True)
+    pts_files = sorted(f for f in os.listdir(pts_dir_abs)
+                       if os.path.isfile(os.path.join(pts_dir_abs, f)) and f[-4:] == '.xyz')
+    for pts_file in pts_files:
+        pts_file_abs = os.path.join(pts_dir_abs, pts_file)
+        mesh_abs = os.path.join(recon_mesh_dir_abs, pts_file[:-4] + '.ply')
+        if not sdf._call_necessary([pts_file_abs], [mesh_abs]):
+            continue
+        xyz = np.loadtxt(pts_file_abs, dtype=np.float64, ndmin=2)
+        if xyz.shape[1] < 6:
+            raise ValueError('{}: Screened Poisson needs points with normals (x y z nx ny nz)'.format(pts_file_abs))
+        verts, faces, _ = poisson.reconstruct(xyz[:, :3], xyz[:, 3:6], **params)
+        mesh_io.write_ply(mesh_abs, verts, faces)
+
+
 def main(argv=None):
     parser = argparse.ArgumentParser(description='Ground-truth point normals (06_normals) for the point clouds in '
                                                  'DATASET_DIR/04_pts from the meshes in DATASET_DIR/03_meshes.')
     parser.add_argument('dataset_dir', help='dataset directory containing 03_meshes and 04_pts')
+    parser.add_argument('--spsr', action='store_true',
+                        help='also reconstruct Screened Poisson surfaces from the ground-truth normals on the GPU '
+                             '(06_poisson_rec_gt_normals) and compare them with 03_meshes for the shapes in valset.txt '
+                             '(comp_poisson_rec_gt_normals.csv)')
     args = parser.parse_args(argv)
     dataset = os.path.abspath(args.dataset_dir)
-    print('### Screened-Poisson reconstructions (06_poisson_rec*) need meshlabserver: skipped')
+    base_dir, dataset_dir = os.path.dirname(dataset), os.path.basename(dataset)
+    if args.spsr:
+        print('### Screened-Poisson reconstruction from PCPNet normals (06_poisson_rec_pcpnet_normals) needs '
+              'PCPNet\'s normals: skipped')
+    else:
+        print('### Screened-Poisson reconstructions (06_poisson_rec*) need meshlabserver: skipped')
     print('### get ground truth normals for point cloud')
-    get_pts_normals(base_dir=os.path.dirname(dataset), dataset_dir=os.path.basename(dataset),
+    get_pts_normals(base_dir=base_dir, dataset_dir=dataset_dir,
                     dir_in_pointcloud='04_pts', dir_in_meshes='03_meshes', dir_out_normals='06_normals',
                     samples_per_model=100000)
+    if not args.spsr:
+        return
+    print('### poisson reconstruction from gt normals')
+    apply_meshlab_filter(base_dir=base_dir, dataset_dir=dataset_dir, pts_dir='06_normals/pts',
+                         recon_mesh_dir='06_poisson_rec_gt_normals', num_processes=1,
+                         filter_file='poisson.mlx', meshlabserver_bin=None)
+    print('### normal estimation and poisson reconstruction gt normals - hausdorff distance')
+    evaluation.mesh_comparison(new_meshes_dir_abs=os.path.join(dataset, '06_poisson_rec_gt_normals'),
+                               ref_meshes_dir_abs=os.path.join(dataset, '03_meshes'), num_processes=1,
+                               report_name=os.path.join(dataset, 'comp_poisson_rec_gt_normals.csv'),
+                               samples_per_model=10000, dataset_file_abs=os.path.join(dataset, 'valset.txt'))
 
 
 if __name__ == '__main__':

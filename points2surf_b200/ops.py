@@ -338,6 +338,30 @@ def mesh_clean(verts, faces):
     return vout[:rep.vertices_out], fout[:rep.faces_out], report
 
 
+def poisson_solve(pts, normals, depth=8, point_weight=4.0, scale=1.1, iters=8):
+    """Screened Poisson solve on the dense (2^depth + 1)^3 node grid (system, solver and deviations from PoissonRecon in
+    include/p2s_b200.h).  pts, normals [N,3] fp32; zero normals drop their point.
+    -> (values [R,R,R] fp32 = iso - chi, positive inside, zero on the surface; report dict of p2s_poisson_report with
+    origin as a tuple and stage_ms as a list).  Node (i, j, k) lies at origin + edge * (i, j, k) / 2^depth."""
+    pts = _dev(pts, torch.float32, 'pts')
+    nrm = _dev(normals, torch.float32, 'normals')
+    if pts.dim() != 2 or pts.shape[1] != 3 or nrm.shape != pts.shape:
+        raise P2SError('pts and normals must have the same shape [N, 3]')
+    cfg = _lib.PoissonConfig(int(depth), float(point_weight), float(scale), int(iters))
+    rep = _lib.PoissonReport()
+    lib = _lib.load()
+    with torch.cuda.device(pts.device):
+        check(lib.p2s_poisson_solve_dev(None, None, 0, C.byref(cfg), None, 0, C.byref(rep), _stream()))
+        R = rep.grid_res
+        values = torch.empty((R, R, R), dtype=torch.float32, device=pts.device)
+        check(lib.p2s_poisson_solve_dev(_ptr(pts), _ptr(nrm), pts.shape[0], C.byref(cfg), _ptr(values), values.numel(),
+                                        C.byref(rep), _stream()))
+    report = {name: getattr(rep, name) for name, _ in _lib.PoissonReport._fields_ if name != 'reserved'}
+    report['origin'] = tuple(rep.origin)
+    report['stage_ms'] = list(rep.stage_ms)
+    return values, report
+
+
 SCANNER_DEFAULTS = dict(res_x=176, res_y=144, lens_angle_w=43.6, lens_angle_h=34.6, max_distance=10.0, noise_mu=0.0)
 
 
