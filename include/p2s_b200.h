@@ -16,6 +16,15 @@
  *     and return after the result is in the host buffer.
  *   - all float data is IEEE fp32, all index data int32, row-major, densely packed.
  *   - there is no CPU fallback anywhere behind this ABI.
+ *
+ * Scratch memory
+ *   Device scratch of the library is kept per (entry point, device, calling thread), grows only, and is
+ *   reused by the next call in stream order.  Calls to one entry point from one thread on two streams are
+ *   therefore not independent: order them (or use one thread per stream).  Under CUDA graph capture:
+ *   - a call whose scratch would have to grow while its stream is capturing fails with an error before it
+ *     enqueues anything; make an eager call of the same size first;
+ *   - scratch handed out during a capture is never freed: when a later eager call needs more, it gets new
+ *     memory and the captured graph keeps the old one for the rest of the process.
  */
 #ifndef P2S_B200_H
 #define P2S_B200_H

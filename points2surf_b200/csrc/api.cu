@@ -28,7 +28,7 @@ void marching_cubes(const float* vol, int res, float level, float* verts, int64_
 #include <map>
 namespace p2s {
 static std::map<std::string, std::pair<double, long>> g_stage;
-bool StageTimer::enabled() { static int e = -1; if (e < 0) { const char* v = getenv("P2S_STAGE_TIMING"); e = (v && v[0] == '1') ? 1 : 0; } return e == 1; }
+bool StageTimer::enabled() { static const bool e = env_flag("P2S_STAGE_TIMING"); return e; }
 void StageTimer::add(const char* label, double ms) { auto& x = g_stage[label]; x.first += ms; x.second += 1; }
 void StageTimer::report() {
     if (!enabled() || g_stage.empty()) return;

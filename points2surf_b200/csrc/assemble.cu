@@ -983,8 +983,10 @@ __global__ void gather_points_kernel(const float* __restrict__ pts, const int32_
 
 }  // namespace
 
+// the device error flag of the patch and sub-sample kernels: one int per device and thread, zero until a kernel sets it
 static int* err_flag_dev() {
-    static thread_local int* flag = nullptr;
+    static thread_local std::vector<int*> flags;
+    int*& flag = for_device(flags);
     if (!flag) {
         P2S_CUDA(cudaMalloc(&flag, sizeof(int)));
         P2S_CUDA(cudaMemset(flag, 0, sizeof(int)));
@@ -995,10 +997,8 @@ static int* err_flag_dev() {
 void gather_points(const float* pts, const int32_t* ids, int64_t count, float* out, cudaStream_t st);
 
 int assemble_error_check(cudaStream_t st) {  // sync; returns and clears the device error flag
-    int h = 0;
     int* f = err_flag_dev();
-    P2S_CUDA(cudaMemcpyAsync(&h, f, sizeof(int), cudaMemcpyDeviceToHost, st));
-    P2S_CUDA(cudaStreamSynchronize(st));
+    const int h = read_back(f, 1, st)[0];
     if (h) P2S_CUDA(cudaMemsetAsync(f, 0, sizeof(int), st));
     return h;
 }
@@ -1012,16 +1012,16 @@ void knn_patch(const float* pts, int64_t N, const float* queries, int64_t Q, int
     // Run length: with 8 queries per CTA a batch of 8 192 queries is 1 024 CTAs = 1.4 waves of the 740 co-resident CTAs, i.e.
     // two waves with the second 38 % full.  Lengthen the runs so that the whole batch is ONE wave (longer runs also amortise
     // the histogram selection of a run's first query better).
-    static thread_local int slots_small = 0, slots_big = 0;
-    if (!slots_small) {
-        int dev = 0, sms = 0, a = 0, b = 0;
-        P2S_CUDA(cudaGetDevice(&dev));
-        P2S_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+    static thread_local std::vector<std::pair<int, int>> t_slots;   // co-resident CTAs (small, big) per device
+    auto& occ = for_device(t_slots);
+    if (!occ.first) {
+        const int sms = sm_count();
+        int a = 0, b = 0;
         P2S_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&a, knn_patch_kernel<kCap>, kThreads, 0));
         P2S_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b, knn_patch_kernel<kCapBig>, kThreads, 0));
-        slots_small = sms * (a > 0 ? a : 1); slots_big = sms * (b > 0 ? b : 1);
+        occ = {sms * (a > 0 ? a : 1), sms * (b > 0 ? b : 1)};
     }
-    const int slots = k <= 512 ? slots_small : slots_big;
+    const int slots = k <= 512 ? occ.first : occ.second;
     int run = (int)cdiv(Q, slots);
     if (run < kRun) run = kRun;
     if (run > 64) run = 64;
@@ -1044,38 +1044,28 @@ void ball_patch(const float* pts, int64_t N, const float* queries, int64_t Q, in
 // their id order, so the result is deterministic) -> per-cell ranges, sorted points, tight boxes.  The index lives in a
 // thread-local workspace and is valid until the next call on this thread (stream order).
 bool cloud_index_usable(int64_t N, int S, int mode) {
-    static int off = -1;
-    if (off < 0) { const char* e = getenv("P2S_SUBSAMPLE_NOCELLS"); off = (e && e[0] == '1') ? 1 : 0; }
+    static const bool off = env_flag("P2S_SUBSAMPLE_NOCELLS");
     return !off && mode == P2S_SUBSAMPLE_WEIGHTED && N >= 2 * (int64_t)S && (size_t)N * 4 <= 150 * 1024;
 }
 
 const CloudIndex* cloud_index_build(const float* pts, int64_t N, cudaStream_t st) {
-    static thread_local DevBuf ws;
+    static thread_local std::vector<Workspace> t_ws;
     static thread_local CloudIndex ci;
+    Workspace& ws = for_device(t_ws).begin(st);
     const int n = (int)N;
-    size_t cub_bytes = 0;
-    P2S_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, cub_bytes, (const uint32_t*)nullptr, (uint32_t*)nullptr, (const int32_t*)nullptr, (int32_t*)nullptr, n, 0, 11, st));
-    auto al = [](size_t b) { return (b + 255) & ~(size_t)255; };
-    size_t off = 0;
-    const size_t o_meta = off; off += al(6 * 4);
-    const size_t o_key = off; off += al((size_t)n * 4);
-    const size_t o_val = off; off += al((size_t)n * 4);
-    const size_t o_keys = off; off += al((size_t)n * 4);
-    const size_t o_perm = off; off += al((size_t)n * 4);
-    const size_t o_start = off; off += al((size_t)(kCC + 1) * 4);
-    const size_t o_spts = off; off += al((size_t)n * 12);
-    const size_t o_cbox = off; off += al((size_t)kCC * 24);
-    const size_t o_cub = off; off += al(cub_bytes);
-    uint8_t* b = (uint8_t*)ws.get(off);
-    float* meta = (float*)(b + o_meta);
-    uint32_t* key = (uint32_t*)(b + o_key); int32_t* val = (int32_t*)(b + o_val);
-    uint32_t* key_s = (uint32_t*)(b + o_keys); int32_t* perm = (int32_t*)(b + o_perm);
+    float* meta = ws.get<float>(6);
+    uint32_t* key = ws.get<uint32_t>(n); int32_t* val = ws.get<int32_t>(n);
+    uint32_t* key_s = ws.get<uint32_t>(n); int32_t* perm = ws.get<int32_t>(n);
+    int32_t* start = ws.get<int32_t>(kCC + 1);
+    float* spts = ws.get<float>(3 * (int64_t)n);
+    float* cbox = ws.get<float>(6 * kCC);
     P2S_LAUNCH(ci_bbox_kernel, 1, 1024, 0, st, pts, n, meta);
     P2S_LAUNCH(ci_key_kernel, (unsigned)cdiv(n, 256), 256, 0, st, pts, n, meta, key, val);
-    P2S_CUDA(cub::DeviceRadixSort::SortPairs(b + o_cub, cub_bytes, key, key_s, val, perm, n, 0, 11, st));    // kCC = 1728 < 2^11
-    g_launches.fetch_add(3, std::memory_order_relaxed);
-    P2S_LAUNCH(ci_finish_kernel, (unsigned)cdiv(kCC + 1, 128), 128, 0, st, pts, n, key_s, perm, (int32_t*)(b + o_start), (float*)(b + o_spts), (float*)(b + o_cbox));
-    ci.meta = meta; ci.spts = (const float*)(b + o_spts); ci.perm = perm; ci.start = (const int32_t*)(b + o_start); ci.cbox = (const float*)(b + o_cbox);
+    cub_run(ws, 3, [&](void* t, size_t& b) {   // kCC = 1728 < 2^11
+        return cub::DeviceRadixSort::SortPairs(t, b, key, key_s, val, perm, n, 0, 11, st);
+    });
+    P2S_LAUNCH(ci_finish_kernel, (unsigned)cdiv(kCC + 1, 128), 128, 0, st, pts, n, key_s, perm, start, spts, cbox);
+    ci.meta = meta; ci.spts = spts; ci.perm = perm; ci.start = start; ci.cbox = cbox;
     return &ci;
 }
 
@@ -1093,32 +1083,19 @@ void subsample(const float* pts, int64_t N, const float* queries, int64_t Q, int
         P2S_LAUNCH(subsample_uniform_kernel, (unsigned)cdiv(threads, 256), 256, 0, st, (int)N, Q, qbase, qidx, S, seed, out);
     } else if (mode == P2S_SUBSAMPLE_WEIGHTED) {
         const size_t cache_bytes = (size_t)N * sizeof(float);
-        static int no_reject = -1;
-        if (no_reject < 0) { const char* e = getenv("P2S_SUBSAMPLE_CLOCKS"); no_reject = (e && e[0] == '1') ? 1 : 0; }
+        static const bool no_reject = env_flag("P2S_SUBSAMPLE_CLOCKS");
         if (cloud_index_usable(N, S, mode) && !no_reject) {
             if (!cidx) cidx = cloud_index_build(pts, N, st);
-            static thread_local bool attr_set = false;
-            if (!attr_set) {
-                P2S_CUDA(cudaFuncSetAttribute(subsample_cells_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 150 * 1024));
-                attr_set = true;
-            }
+            set_smem_attr_once(subsample_cells_kernel, 150 * 1024);
             P2S_LAUNCH(subsample_cells_kernel, (unsigned)Q, kThreads, cache_bytes, st, *cidx, (int)N, queries, qbase, qidx, S, seed, out, pts_out, err_flag_dev());
             gathered = true;
         } else if (cache_bytes <= 160 * 1024 && N >= 2 * (int64_t)S && !no_reject) {
             // rejection sampling: cheap when at most half of the cloud is drawn (the acceptance rate is >= 0.05 by construction)
-            static thread_local bool attr_set = false;
-            if (!attr_set) {
-                P2S_CUDA(cudaFuncSetAttribute(subsample_reject_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));
-                attr_set = true;
-            }
+            set_smem_attr_once(subsample_reject_kernel, 160 * 1024);
             P2S_LAUNCH(subsample_reject_kernel, (unsigned)Q, kThreads, cache_bytes, st, pts, (int)N, queries, qbase, qidx, S, seed, out, pts_out, err_flag_dev());
             gathered = true;
         } else if (cache_bytes <= 160 * 1024) {
-            static thread_local bool attr_set = false;
-            if (!attr_set) {
-                P2S_CUDA(cudaFuncSetAttribute(subsample_weighted_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));
-                attr_set = true;
-            }
+            set_smem_attr_once(subsample_weighted_kernel<true>, 160 * 1024);
             P2S_LAUNCH(subsample_weighted_kernel<true>, (unsigned)Q, kThreads, cache_bytes, st, pts, (int)N, queries, qbase, qidx, S, seed, out, err_flag_dev());
         } else {
             P2S_LAUNCH(subsample_weighted_kernel<false>, (unsigned)Q, kThreads, 0, st, pts, (int)N, queries, qbase, qidx, S, seed, out, err_flag_dev());

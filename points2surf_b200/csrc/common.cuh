@@ -7,7 +7,9 @@
 #include <cstring>
 #include <string>
 #include <stdexcept>
+#include <algorithm>
 #include <atomic>
+#include <set>
 #include <vector>
 
 #include "../../include/p2s_b200.h"
@@ -76,18 +78,24 @@ struct StageScope {
     ~StageScope();
 };
 
-// grow-only device scratch buffer
+// grow-only device scratch buffer.  `capturing`: the caller's stream is capturing a CUDA graph, which then holds p, so p
+// may not move now and is never freed later (it stays allocated for the rest of the process).
 struct DevBuf {
     void* p = nullptr;
     size_t bytes = 0;
-    void* get(size_t need) {
+    bool captured = false;
+    void* get(size_t need, bool capturing = false) {
         if (need > bytes) {
-            if (p) P2S_CUDA(cudaFree(p));
+            P2S_CHECK(!capturing, "library scratch would have to grow while the stream is capturing a CUDA graph: make an "
+                                  "eager call of the same size first");
+            if (p && !captured) P2S_CUDA(cudaFree(p));
             p = nullptr;
+            captured = false;
             size_t want = need + need / 8;
             P2S_CUDA(cudaMalloc(&p, want));
             bytes = want;
         }
+        captured = captured || capturing;
         return p;
     }
     template <class T>
@@ -98,6 +106,93 @@ struct DevBuf {
         bytes = 0;
     }
 };
+
+// v[current device]; v is sized to the device count on first use
+template <class T>
+T& for_device(std::vector<T>& v) {
+    if (v.empty()) {
+        int n = 0;
+        P2S_CUDA(cudaGetDeviceCount(&n));
+        v.resize(n);
+    }
+    int d = 0;
+    P2S_CUDA(cudaGetDevice(&d));
+    return v.at(d);
+}
+
+// Library scratch (the rules are in include/p2s_b200.h, "Scratch memory").  Every entry point keeps one
+// `static thread_local std::vector<Workspace>` and starts each call with `for_device(ws).begin(st)`.  Buffers are handed
+// out in request order, so the same sequence of requests reuses the same buffers; mark()/rewind() let a helper called
+// more than once reuse its own slots.  CUB's temporary storage is one more grow-only buffer (cub_run).
+struct Workspace {
+    std::vector<DevBuf> bufs;
+    DevBuf cub;
+    size_t next = 0;
+    cudaStream_t st = nullptr;
+
+    Workspace& begin(cudaStream_t s) {
+        next = 0;
+        st = s;
+        return *this;
+    }
+    void* grow(DevBuf& b, size_t bytes) {
+        cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+        P2S_CUDA(cudaStreamIsCapturing(st, &cs));
+        return b.get(bytes, cs != cudaStreamCaptureStatusNone);
+    }
+    template <class T>
+    T* get(int64_t count) {
+        if (next == bufs.size()) bufs.emplace_back();
+        return reinterpret_cast<T*>(grow(bufs[next++], (size_t)std::max<int64_t>(count, 1) * sizeof(T)));
+    }
+    size_t mark() const { return next; }
+    void rewind(size_t m) { next = m; }
+};
+
+// runs a CUB device algorithm: size query, grow the workspace's CUB storage, call.  `counted`: what the call adds to
+// p2s_launch_count(), whatever CUB launches.
+template <class Fn>
+void cub_run(Workspace& ws, int counted, Fn fn) {
+    size_t bytes = 0;
+    P2S_CUDA(fn(nullptr, bytes));
+    P2S_CUDA(fn(ws.grow(ws.cub, std::max<size_t>(bytes, 16)), bytes));
+    g_launches.fetch_add(counted, std::memory_order_relaxed);
+}
+
+// copies n values to the host and waits for the stream
+template <class T>
+std::vector<T> read_back(const T* dev, size_t n, cudaStream_t st) {
+    std::vector<T> h(n);
+    P2S_CUDA(cudaMemcpyAsync(h.data(), dev, n * sizeof(T), cudaMemcpyDeviceToHost, st));
+    P2S_CUDA(cudaStreamSynchronize(st));
+    return h;
+}
+
+static inline unsigned grid1d(int64_t n, int threads) { return (unsigned)cdiv(std::max<int64_t>(n, 1), threads); }
+
+static inline int sm_count() {   // of the current device
+    int d = 0, n = 0;
+    P2S_CUDA(cudaGetDevice(&d));
+    P2S_CUDA(cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, d));
+    return n;
+}
+
+// raises the kernel's dynamic shared-memory limit to `bytes` on the current device, once per device and thread
+template <class K>
+void set_smem_attr_once(K* kernel, size_t bytes) {
+    static thread_local std::set<std::pair<const void*, int>> done;   // (kernel, device)
+    int d = 0;
+    P2S_CUDA(cudaGetDevice(&d));
+    if (done.count({(const void*)kernel, d})) return;
+    P2S_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
+    done.insert({(const void*)kernel, d});
+}
+
+// true when the environment variable starts with '1'; call sites that read it once keep it in a static
+static inline bool env_flag(const char* name) {
+    const char* e = getenv(name);
+    return e && e[0] == '1';
+}
 
 // ---- Philox4x32-10 (Salmon et al. 2011), counter-based: (key, counter) -> 4 x u32 ----
 __host__ __device__ inline void philox4x32_10(uint32_t k0, uint32_t k1, uint32_t c0, uint32_t c1,

@@ -277,12 +277,8 @@ uint8_t* fc_tc_pack(const Layer& L, std::vector<void*>& allocs) {
 }
 
 void fc_tc_init() {
-    static bool done = false;
-    if (!done) {
-        P2S_CUDA(cudaFuncSetAttribute(fc_tc_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFcSmem));
-        P2S_CUDA(cudaFuncSetAttribute(fc_tc_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFcSmem));
-        done = true;
-    }
+    set_smem_attr_once(fc_tc_kernel<false>, kFcSmem);
+    set_smem_attr_once(fc_tc_kernel<true>, kFcSmem);
 }
 
 void launch_fc_tc(const float* A, int lda, const uint8_t* Wimg, const float* bias, float* C, int ldc,
@@ -389,11 +385,8 @@ void launch_absmax_cols(const float* X, int ld, int64_t rows, int cols, unsigned
     P2S_CHECK(cols % 4 == 0 && ld % 4 == 0 && (uintptr_t)X % 16 == 0, "absmax_cols: unaligned rows");
     P2S_CUDA(cudaMemsetAsync(out, 0, sizeof(unsigned) * (size_t)cols, st));
     if (rows <= 0) return;
-    int dev = 0, sms = 132;
-    P2S_CUDA(cudaGetDevice(&dev));
-    P2S_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
     const int64_t cb = cdiv(cols, 128);
-    const int64_t slices = std::min<int64_t>(cdiv(rows, 64), std::max<int64_t>(1, cdiv(8 * (int64_t)sms, cb)));
+    const int64_t slices = std::min<int64_t>(cdiv(rows, 64), std::max<int64_t>(1, cdiv(8 * (int64_t)sm_count(), cb)));
     P2S_LAUNCH(absmax_cols_kernel, dim3((unsigned)cb, (unsigned)std::min<int64_t>(slices, 65535)), 256, 0, st, X, ld, rows, cols, out);
 }
 
@@ -403,31 +396,26 @@ void launch_absmax_cols(const float* X, int ld, int64_t rows, int cols, unsigned
 // Every output element meets |C - C_exact| <= gamma_K sum_k |a_k b_k| + 2^-40 K max_k |a_k| max_k |b_k| (up to the
 // tensor cores' accumulation order) at any operand scale inside fp32's normal range.
 bool gemm_nt_tc_ok(const float* A, int lda, const float* C, int ldc, int64_t M, int N, int K) {
-    static int disabled = -1;
-    if (disabled < 0) {
-        const char* e = getenv("P2S_TRAIN_GEMM_FP32");
-        disabled = (e && e[0] == '1') ? 1 : 0;
-    }
+    static const bool disabled = env_flag("P2S_TRAIN_GEMM_FP32");
     return !disabled && N % 4 == 0 && N >= 64 && K % kBK == 0 && K >= kBK && N <= 4096 && M >= 128 && M < (int64_t)1 << 31 && lda % 4 == 0 && ldc % 4 == 0 &&
            ((uintptr_t)A % 16 == 0) && ((uintptr_t)C % 16 == 0);
 }
 
 void launch_gemm_nt_tc(const float* A, int lda, const float* W, const float* bias, float* C, int ldc, int64_t M, int N,
                        int K, bool relu, cudaStream_t st) {
-    static thread_local DevBuf img, zeros, amax;
-    static thread_local bool zeroed = false;
-    fc_tc_init();
+    static thread_local std::vector<Workspace> t_ws;
+    static thread_local std::vector<DevBuf> t_zeros;   // 4096 zeros per device: the bias of calls without one
+    Workspace& ws = for_device(t_ws).begin(st);
     const int Npad = (int)(cdiv(N, 128) * 128);
-    uint8_t* wimg = reinterpret_cast<uint8_t*>(img.get((size_t)Npad * K * 4));
-    int* a_exp = amax.as<int>((size_t)M + N + 2);
+    uint8_t* wimg = ws.get<uint8_t>((int64_t)Npad * K * 4);
+    int* a_exp = ws.get<int>(M + N + 2);
     int* w_exp = a_exp + ((M + 1) & ~(int64_t)1);          // 8-byte aligned: the epilogue reads column pairs
+    fc_tc_init();
     if (!bias) {
-        float* z = zeros.as<float>(4096);
-        if (!zeroed) {
-            P2S_CUDA(cudaMemsetAsync(z, 0, 4096 * sizeof(float), st));
-            zeroed = true;
-        }
-        bias = z;
+        DevBuf& z = for_device(t_zeros);
+        const bool fresh = !z.p;
+        bias = reinterpret_cast<float*>(ws.grow(z, 4096 * sizeof(float)));
+        if (fresh) P2S_CUDA(cudaMemsetAsync(z.p, 0, 4096 * sizeof(float), st));
     }
     launch_split_exp_rows(A, lda, M, K, a_exp, st);
     launch_split_exp_rows(W, K, N, K, w_exp, st);

@@ -151,11 +151,7 @@ gemm_tn_tc_kernel(const float* __restrict__ A, int lda, const float* __restrict_
 }  // namespace
 
 bool gemm_tn_tc_ok(const float* A, int lda, const float* B, int ldb, int64_t M, int N, int K) {
-    static int disabled = -1;
-    if (disabled < 0) {
-        const char* e = getenv("P2S_TRAIN_GEMM_FP32");
-        disabled = (e && e[0] == '1') ? 1 : 0;
-    }
+    static const bool disabled = env_flag("P2S_TRAIN_GEMM_FP32");
     return !disabled && M >= 4096 && N >= 64 && K >= 64 && N % 4 == 0 && K % 4 == 0 && lda % 4 == 0 && ldb % 4 == 0 &&
            ((uintptr_t)A % 16 == 0) && ((uintptr_t)B % 16 == 0);
 }
@@ -163,20 +159,13 @@ bool gemm_tn_tc_ok(const float* A, int lda, const float* B, int ldb, int64_t M, 
 // C must already hold the values the product is added to (zeros or a running gradient)
 void launch_gemm_tn_tc(const float* A, int lda, const float* B, int ldb, float* C, int ldc, int64_t M, int N, int K,
                        cudaStream_t st) {
-    static bool attr = false;
-    if (!attr) {
-        P2S_CUDA(cudaFuncSetAttribute(gemm_tn_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmem));
-        attr = true;
-    }
-    static thread_local DevBuf amax;
-    unsigned* a_amax = amax.as<unsigned>((size_t)N + K);
+    static thread_local std::vector<Workspace> t_ws;
+    unsigned* a_amax = for_device(t_ws).begin(st).get<unsigned>((int64_t)N + K);
+    set_smem_attr_once(gemm_tn_tc_kernel, kSmem);
     launch_absmax_cols(A, lda, M, N, a_amax, st);
     launch_absmax_cols(B, ldb, M, K, a_amax + N, st);
-    int dev = 0, sms = 132;
-    P2S_CUDA(cudaGetDevice(&dev));
-    P2S_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
     const int64_t tiles = cdiv(N, 128) * cdiv(K, 128);
-    int64_t splits = std::max<int64_t>(1, cdiv(2 * (int64_t)sms, tiles));
+    int64_t splits = std::max<int64_t>(1, cdiv(2 * (int64_t)sm_count(), tiles));
     splits = std::min<int64_t>(splits, cdiv(M, 1024));
     splits = std::min<int64_t>(splits, 65535);
     int64_t rows = cdiv(cdiv(M, splits), kBM) * kBM;

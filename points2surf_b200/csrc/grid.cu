@@ -65,36 +65,25 @@ __global__ void query_points_kernel(const int32_t* __restrict__ lin, int64_t Q, 
     out[i * 3 + 2] = (float)(((double)iz + 0.5) / (double)res * 2.0 - 1.0);
 }
 
-static thread_local DevBuf t_grid_ws;
-
 void query_grid(const float* pts, int64_t N, int res, int eps, int32_t* lin_idx, int64_t cap,
                 int64_t* count_host, cudaStream_t st) {
     P2S_CHECK(res >= 2 && res <= 1024, "grid resolution out of range");
     P2S_CHECK(eps >= 1 && eps <= 31, "epsilon out of range");
     const int64_t vox = (int64_t)res * res * res;
-    size_t cub_bytes = 0;
-    cub::CountingInputIterator<int32_t> counting(0);
-    int* d_num = nullptr;
-    cub::DeviceSelect::Flagged(nullptr, cub_bytes, counting, (uint8_t*)nullptr, (int32_t*)nullptr, d_num, (int)vox, st);
-    size_t off_flag = (size_t)vox, off_sel = off_flag + (size_t)vox;
-    off_sel = (off_sel + 255) / 256 * 256;
-    size_t off_num = off_sel + (size_t)vox * 4;
-    size_t off_cub = off_num + 256;
-    uint8_t* base = (uint8_t*)t_grid_ws.get(off_cub + cub_bytes);
-    uint8_t* occ = base;
-    uint8_t* flag = base + off_flag;
-    int32_t* sel = (int32_t*)(base + off_sel);
-    d_num = (int*)(base + off_num);
+    static thread_local std::vector<Workspace> t_ws;
+    Workspace& ws = for_device(t_ws).begin(st);
+    uint8_t* occ = ws.get<uint8_t>(vox);
+    uint8_t* flag = ws.get<uint8_t>(vox);
+    int32_t* sel = ws.get<int32_t>(vox);
+    int* d_num = ws.get<int>(1);
     P2S_CUDA(cudaMemsetAsync(occ, 0, (size_t)vox, st));
     P2S_LAUNCH(occupancy_kernel, (unsigned)cdiv(N, 256), 256, 0, st, pts, N, res, occ);
     const int lo = -((eps + 1) / 2) + 1, hi = eps / 2;
     const int64_t threads = (int64_t)res * res * ((res + 3) / 4);
     P2S_LAUNCH(dilate_flag_kernel, (unsigned)cdiv(threads, 256), 256, 0, st, occ, res, lo, hi, flag);
-    P2S_CUDA(cub::DeviceSelect::Flagged(base + off_cub, cub_bytes, counting, flag, sel, d_num, (int)vox, st));
-    g_launches.fetch_add(2, std::memory_order_relaxed);  // cub: scan + select kernels
-    int h_num = 0;
-    P2S_CUDA(cudaMemcpyAsync(&h_num, d_num, sizeof(int), cudaMemcpyDeviceToHost, st));
-    P2S_CUDA(cudaStreamSynchronize(st));
+    cub::CountingInputIterator<int32_t> counting(0);
+    cub_run(ws, 2, [&](void* t, size_t& b) { return cub::DeviceSelect::Flagged(t, b, counting, flag, sel, d_num, (int)vox, st); });
+    const int h_num = read_back(d_num, 1, st)[0];
     *count_host = h_num;
     int64_t ncopy = h_num < cap ? h_num : cap;
     if (ncopy > 0) P2S_CUDA(cudaMemcpyAsync(lin_idx, sel, (size_t)ncopy * 4, cudaMemcpyDeviceToDevice, st));

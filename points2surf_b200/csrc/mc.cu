@@ -140,8 +140,6 @@ __global__ void mc_flip_kernel(int32_t* __restrict__ faces, int64_t F, const dou
     faces[i * 3 + 2] = t;
 }
 
-thread_local DevBuf t_mc_ws;
-
 }  // namespace
 
 void marching_cubes(const float* vol, int R, float level, float* verts, int64_t vcap, int32_t* faces, int64_t fcap,
@@ -150,25 +148,18 @@ void marching_cubes(const float* vol, int R, float level, float* verts, int64_t 
     const int64_t V = (int64_t)R * R * R, E = 3 * V;
     const int64_t C = (int64_t)(R - 1) * (R - 1) * (R - 1);
     P2S_CHECK(E < (1ll << 31), "volume too large for 32-bit edge ids");
-    size_t cub1 = 0, cub2 = 0;
-    cub::DeviceScan::ExclusiveSum(nullptr, cub1, (uint8_t*)nullptr, (int32_t*)nullptr, (int)E, st);
-    cub::DeviceScan::ExclusiveSum(nullptr, cub2, (uint8_t*)nullptr, (int32_t*)nullptr, (int)C, st);
-    size_t cub_bytes = cub1 > cub2 ? cub1 : cub2;
-    auto al = [](size_t x) { return (x + 255) / 256 * 256; };
-    size_t off_flags = 256, off_vid = off_flags + al(E), off_cnt = off_vid + al(E * 4), off_offs = off_cnt + al(C),
-           off_cub = off_offs + al(C * 4);
-    uint8_t* base = (uint8_t*)t_mc_ws.get(off_cub + cub_bytes);
-    double* acc = (double*)base;
-    uint8_t* flags = base + off_flags;
-    int32_t* vid = (int32_t*)(base + off_vid);
-    uint8_t* counts = base + off_cnt;
-    int32_t* offs = (int32_t*)(base + off_offs);
+    static thread_local std::vector<Workspace> t_ws;
+    Workspace& ws = for_device(t_ws).begin(st);
+    double* acc = ws.get<double>(1);
+    uint8_t* flags = ws.get<uint8_t>(E);
+    int32_t* vid = ws.get<int32_t>(E);
+    uint8_t* counts = ws.get<uint8_t>(C);
+    int32_t* offs = ws.get<int32_t>(C);
 
     P2S_LAUNCH(mc_edge_flags_kernel, (unsigned)cdiv(V, 256), 256, 0, st, vol, R, level, flags);
-    P2S_CUDA(cub::DeviceScan::ExclusiveSum(base + off_cub, cub_bytes, flags, vid, (int)E, st));
+    cub_run(ws, 2, [&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, flags, vid, (int)E, st); });
     P2S_LAUNCH(mc_cell_count_kernel, (unsigned)cdiv(C, 256), 256, 0, st, vol, R, level, counts);
-    P2S_CUDA(cub::DeviceScan::ExclusiveSum(base + off_cub, cub_bytes, counts, offs, (int)C, st));
-    g_launches.fetch_add(4, std::memory_order_relaxed);  // cub: 2 kernels per scan
+    cub_run(ws, 2, [&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, counts, offs, (int)C, st); });
     int32_t last_vid = 0, last_off = 0;
     uint8_t last_flag = 0, last_cnt = 0;
     P2S_CUDA(cudaMemcpyAsync(&last_vid, vid + (E - 1), 4, cudaMemcpyDeviceToHost, st));

@@ -426,36 +426,6 @@ struct MaxOp {
     __device__ __forceinline__ int32_t operator()(int32_t a, int32_t b) const { return a > b ? a : b; }
 };
 
-struct Scratch {
-    DevBuf cnt, kx, ky, kz, kt, kg, finite, ord0, ord1, headpos, runstart, rep, cand, ids0, ids1, dkey0, dkey1, num, cub;
-    DevBuf W, hkey, hkey_s, hval, hval_s, ukey, rcnt, roff, deg, nb, nfill, foff;
-    DevBuf par, has2, root, parity, nonorient, flip, sel, selroot, selroot_s, sel_s, segroot, segcnt, segoff, det, segsum;
-    DevBuf used, newidx, ccnt;
-};
-Scratch& scratch() {
-    static thread_local Scratch s;
-    return s;
-}
-
-unsigned grid(int64_t n) { return (unsigned)cdiv(std::max<int64_t>(n, 1), 256); }
-
-// runs a CUB device algorithm: size query, grow-only temporary storage, call
-template <class Fn>
-void cub_run(Fn fn) {
-    size_t bytes = 0;
-    P2S_CUDA(fn(nullptr, bytes));
-    P2S_CUDA(fn(scratch().cub.get(std::max<size_t>(bytes, 16)), bytes));
-    g_launches.fetch_add(1, std::memory_order_relaxed);   // counts the CUB call once, whatever it launches
-}
-
-template <class T>
-T read1(const T* dev, cudaStream_t st) {
-    T h;
-    P2S_CUDA(cudaMemcpyAsync(&h, dev, sizeof(T), cudaMemcpyDeviceToHost, st));
-    P2S_CUDA(cudaStreamSynchronize(st));
-    return h;
-}
-
 // the undirected edges of the working faces W [n][3]: sorted half-edges he, runs (count, offset)
 struct Edges {
     int32_t *he, *rcnt, *roff;
@@ -463,32 +433,33 @@ struct Edges {
     long long boundary, nonmanifold, inconsistent;
 };
 
-Edges classify(const int32_t* W, int n, cudaStream_t st) {
-    auto& sc = scratch();
+// its buffers are the workspace slots from `at` on, so that every call reuses the same ones
+Edges classify(Workspace& ws, size_t at, const int32_t* W, int n, cudaStream_t st) {
+    const size_t resume = ws.mark();
+    ws.rewind(at);
     Edges e{};
     const int n3 = 3 * n;
-    unsigned long long* c = sc.ccnt.as<unsigned long long>(C_COUNT);
+    unsigned long long* c = ws.get<unsigned long long>(C_COUNT);
+    auto* key = ws.get<unsigned long long>(n3);
+    auto* key_s = ws.get<unsigned long long>(n3);
+    int32_t* val = ws.get<int32_t>(n3);
+    e.he = ws.get<int32_t>(n3);
+    auto* ukey = ws.get<unsigned long long>(n3);
+    e.rcnt = ws.get<int32_t>(n3);
+    e.roff = ws.get<int32_t>(n3);
+    int* d_num = ws.get<int>(1);
+    ws.rewind(std::max(resume, ws.mark()));
     P2S_CUDA(cudaMemsetAsync(c, 0, C_COUNT * sizeof(unsigned long long), st));
     if (n == 0) return e;
-    auto* key = sc.hkey.as<unsigned long long>(n3);
-    auto* key_s = sc.hkey_s.as<unsigned long long>(n3);
-    int32_t* val = sc.hval.as<int32_t>(n3);
-    e.he = sc.hval_s.as<int32_t>(n3);
-    auto* ukey = sc.ukey.as<unsigned long long>(n3);
-    e.rcnt = sc.rcnt.as<int32_t>(n3);
-    e.roff = sc.roff.as<int32_t>(n3);
-    int* d_num = sc.num.as<int>(1);
-    P2S_LAUNCH(mc_halfedge_kernel, grid(n3), 256, 0, st, W, n3, key, val);
-    cub_run([&](void* t, size_t& b) { return cub::DeviceRadixSort::SortPairs(t, b, key, key_s, val, e.he, n3, 0, 64, st); });
-    cub_run([&](void* t, size_t& b) {
+    P2S_LAUNCH(mc_halfedge_kernel, grid1d(n3, 256), 256, 0, st, W, n3, key, val);
+    cub_run(ws, 1, [&](void* t, size_t& b) { return cub::DeviceRadixSort::SortPairs(t, b, key, key_s, val, e.he, n3, 0, 64, st); });
+    cub_run(ws, 1, [&](void* t, size_t& b) {
         return cub::DeviceRunLengthEncode::Encode(t, b, key_s, ukey, e.rcnt, d_num, n3, st);
     });
-    e.R = read1(d_num, st);
-    cub_run([&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, e.rcnt, e.roff, e.R, st); });
-    P2S_LAUNCH(mc_classify_kernel, grid(e.R), 256, 0, st, W, e.he, e.rcnt, e.roff, e.R, c);
-    unsigned long long h[C_COUNT];
-    P2S_CUDA(cudaMemcpyAsync(h, c, sizeof(h), cudaMemcpyDeviceToHost, st));
-    P2S_CUDA(cudaStreamSynchronize(st));
+    e.R = read_back(d_num, 1, st)[0];
+    cub_run(ws, 1, [&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, e.rcnt, e.roff, e.R, st); });
+    P2S_LAUNCH(mc_classify_kernel, grid1d(e.R, 256), 256, 0, st, W, e.he, e.rcnt, e.roff, e.R, c);
+    const auto h = read_back(c, C_COUNT, st);
     e.boundary = (long long)h[C_BOUNDARY];
     e.nonmanifold = (long long)h[C_NONMANIFOLD];
     e.inconsistent = (long long)h[C_INCONSISTENT];
@@ -496,10 +467,10 @@ Edges classify(const int32_t* W, int n, cudaStream_t st) {
 }
 
 // the fixed-order sum of mc_segment_sum_kernel over d [n]
-double fixed_sum(const double* d, int n, cudaStream_t st) {
-    double* out = scratch().segsum.as<double>(1);
+double fixed_sum(Workspace& ws, const double* d, int n, cudaStream_t st) {
+    double* out = ws.get<double>(1);
     P2S_LAUNCH(mc_segment_sum_kernel, 1, kSumThreads, 0, st, d, nullptr, nullptr, n, out);
-    return read1(out, st);
+    return read_back(out, 1, st)[0];
 }
 
 }  // namespace
@@ -509,68 +480,64 @@ void mesh_clean(const float* verts, int64_t V64, const int32_t* faces, int64_t F
     P2S_CHECK(V64 >= 0 && F64 >= 0 && vcap >= 0 && fcap >= 0, "negative size");
     P2S_CHECK(V64 < INT32_MAX && 2 * F64 < INT32_MAX / 3, "mesh too large for int32 indices");
     const int V = (int)V64, F = (int)F64;
-    auto& sc = scratch();
+    static thread_local std::vector<Workspace> t_ws;
+    Workspace& ws = for_device(t_ws).begin(st);
     p2s_clean_report R{};
     R.vertices_in = V;
     R.faces_in = F;
-    unsigned long long* cnt = sc.cnt.as<unsigned long long>(C_COUNT);
+    unsigned long long* cnt = ws.get<unsigned long long>(C_COUNT);
     P2S_CUDA(cudaMemsetAsync(cnt, 0, C_COUNT * sizeof(unsigned long long), st));
-    auto counters = [&](unsigned long long* h) {
-        P2S_CUDA(cudaMemcpyAsync(h, cnt, C_COUNT * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
-        P2S_CUDA(cudaStreamSynchronize(st));
-    };
-    unsigned long long h[C_COUNT];
 
     // 1. input checks and weld keys
-    long long *kx = sc.kx.as<long long>(V), *ky = sc.ky.as<long long>(V), *kz = sc.kz.as<long long>(V);
-    long long* kt = sc.kt.as<long long>(V);
-    uint8_t* finite = sc.finite.as<uint8_t>(V);
-    int32_t *ord0 = sc.ord0.as<int32_t>(V), *ord1 = sc.ord1.as<int32_t>(V);
-    if (F > 0) P2S_LAUNCH(mc_index_check_kernel, grid(3 * (int64_t)F), 256, 0, st, faces, 3 * (int64_t)F, V64, cnt);
-    if (V > 0) P2S_LAUNCH(mc_vertex_key_kernel, grid(V), 256, 0, st, verts, V, kx, ky, kz, finite, ord0, cnt);
-    counters(h);
+    long long *kx = ws.get<long long>(V), *ky = ws.get<long long>(V), *kz = ws.get<long long>(V);
+    long long* kt = ws.get<long long>(V);
+    uint8_t* finite = ws.get<uint8_t>(V);
+    int32_t *ord0 = ws.get<int32_t>(V), *ord1 = ws.get<int32_t>(V);
+    if (F > 0) P2S_LAUNCH(mc_index_check_kernel, grid1d(3 * (int64_t)F, 256), 256, 0, st, faces, 3 * (int64_t)F, V64, cnt);
+    if (V > 0) P2S_LAUNCH(mc_vertex_key_kernel, grid1d(V, 256), 256, 0, st, verts, V, kx, ky, kz, finite, ord0, cnt);
+    std::vector<unsigned long long> h = read_back(cnt, C_COUNT, st);
     P2S_CHECK(h[C_BAD_INDEX] == 0, "face index outside [0, V)");
     P2S_CHECK(h[C_OVERFLOW] == 0, "finite vertex coordinate with |x| >= 9e10 (weld key overflows int64)");
 
     // 2. weld: stable sorts by z, y, x key leave equal keys adjacent in ascending index order
-    int32_t* rep = sc.rep.as<int32_t>(V);
+    int32_t* rep = ws.get<int32_t>(V);
     if (V > 0) {
-        long long* kg = sc.kg.as<long long>(V);   // keys gathered into the current order
-        cub_run([&](void* t, size_t& b) { return cub::DeviceRadixSort::SortPairs(t, b, kz, kt, ord0, ord1, V, 0, 64, st); });
-        P2S_LAUNCH(mc_gather_kernel<long long>, grid(V), 256, 0, st, ky, ord1, V, kg);
-        cub_run([&](void* t, size_t& b) { return cub::DeviceRadixSort::SortPairs(t, b, kg, kt, ord1, ord0, V, 0, 64, st); });
-        P2S_LAUNCH(mc_gather_kernel<long long>, grid(V), 256, 0, st, kx, ord0, V, kg);
-        cub_run([&](void* t, size_t& b) { return cub::DeviceRadixSort::SortPairs(t, b, kg, kt, ord0, ord1, V, 0, 64, st); });
-        int32_t *headpos = sc.headpos.as<int32_t>(V), *runstart = sc.runstart.as<int32_t>(V);
-        P2S_LAUNCH(mc_weld_head_kernel, grid(V), 256, 0, st, ord1, V, kx, ky, kz, finite, headpos, cnt);
-        cub_run([&](void* t, size_t& b) { return cub::DeviceScan::InclusiveScan(t, b, headpos, runstart, MaxOp(), V, st); });
-        P2S_LAUNCH(mc_weld_rep_kernel, grid(V), 256, 0, st, ord1, runstart, V, rep);
+        long long* kg = ws.get<long long>(V);   // keys gathered into the current order
+        cub_run(ws, 1, [&](void* t, size_t& b) { return cub::DeviceRadixSort::SortPairs(t, b, kz, kt, ord0, ord1, V, 0, 64, st); });
+        P2S_LAUNCH(mc_gather_kernel<long long>, grid1d(V, 256), 256, 0, st, ky, ord1, V, kg);
+        cub_run(ws, 1, [&](void* t, size_t& b) { return cub::DeviceRadixSort::SortPairs(t, b, kg, kt, ord1, ord0, V, 0, 64, st); });
+        P2S_LAUNCH(mc_gather_kernel<long long>, grid1d(V, 256), 256, 0, st, kx, ord0, V, kg);
+        cub_run(ws, 1, [&](void* t, size_t& b) { return cub::DeviceRadixSort::SortPairs(t, b, kg, kt, ord0, ord1, V, 0, 64, st); });
+        int32_t *headpos = ws.get<int32_t>(V), *runstart = ws.get<int32_t>(V);
+        P2S_LAUNCH(mc_weld_head_kernel, grid1d(V, 256), 256, 0, st, ord1, V, kx, ky, kz, finite, headpos, cnt);
+        cub_run(ws, 1, [&](void* t, size_t& b) { return cub::DeviceScan::InclusiveScan(t, b, headpos, runstart, MaxOp(), V, st); });
+        P2S_LAUNCH(mc_weld_rep_kernel, grid1d(V, 256), 256, 0, st, ord1, runstart, V, rep);
     }
 
     // 3. non-finite, degenerate and duplicate faces
-    uint8_t* alive = sc.cand.as<uint8_t>(F);
-    int32_t *ids0 = sc.ids0.as<int32_t>(F), *ids1 = sc.ids1.as<int32_t>(F);
-    int* d_num = sc.num.as<int>(1);
+    uint8_t* alive = ws.get<uint8_t>(F);
+    int32_t *ids0 = ws.get<int32_t>(F), *ids1 = ws.get<int32_t>(F);
+    int* d_num = ws.get<int>(1);
     cub::CountingInputIterator<int32_t> counting(0);
     int A = 0;
     if (F > 0) {
-        P2S_LAUNCH(mc_face_kernel, grid(F), 256, 0, st, verts, faces, F, rep, finite, alive, cnt);
-        cub_run([&](void* t, size_t& b) { return cub::DeviceSelect::Flagged(t, b, counting, alive, ids0, d_num, F, st); });
-        const int C = read1(d_num, st);
+        P2S_LAUNCH(mc_face_kernel, grid1d(F, 256), 256, 0, st, verts, faces, F, rep, finite, alive, cnt);
+        cub_run(ws, 1, [&](void* t, size_t& b) { return cub::DeviceSelect::Flagged(t, b, counting, alive, ids0, d_num, F, st); });
+        const int C = read_back(d_num, 1, st)[0];
         if (C > 1) {
-            auto *k0 = sc.dkey0.as<unsigned long long>(C), *k1 = sc.dkey1.as<unsigned long long>(C);
-            P2S_LAUNCH(mc_dup_key_kernel, grid(C), 256, 0, st, faces, rep, ids0, C, false, k0);
-            cub_run([&](void* t, size_t& b) { return cub::DeviceRadixSort::SortPairs(t, b, k0, k1, ids0, ids1, C, 0, 64, st); });
-            P2S_LAUNCH(mc_dup_key_kernel, grid(C), 256, 0, st, faces, rep, ids1, C, true, k0);
-            cub_run([&](void* t, size_t& b) { return cub::DeviceRadixSort::SortPairs(t, b, k0, k1, ids1, ids0, C, 0, 32, st); });
-            P2S_LAUNCH(mc_dup_mark_kernel, grid(C), 256, 0, st, faces, rep, ids0, C, alive, cnt);
-            cub_run([&](void* t, size_t& b) { return cub::DeviceSelect::Flagged(t, b, counting, alive, ids0, d_num, F, st); });
-            A = read1(d_num, st);
+            auto *k0 = ws.get<unsigned long long>(C), *k1 = ws.get<unsigned long long>(C);
+            P2S_LAUNCH(mc_dup_key_kernel, grid1d(C, 256), 256, 0, st, faces, rep, ids0, C, false, k0);
+            cub_run(ws, 1, [&](void* t, size_t& b) { return cub::DeviceRadixSort::SortPairs(t, b, k0, k1, ids0, ids1, C, 0, 64, st); });
+            P2S_LAUNCH(mc_dup_key_kernel, grid1d(C, 256), 256, 0, st, faces, rep, ids1, C, true, k0);
+            cub_run(ws, 1, [&](void* t, size_t& b) { return cub::DeviceRadixSort::SortPairs(t, b, k0, k1, ids1, ids0, C, 0, 32, st); });
+            P2S_LAUNCH(mc_dup_mark_kernel, grid1d(C, 256), 256, 0, st, faces, rep, ids0, C, alive, cnt);
+            cub_run(ws, 1, [&](void* t, size_t& b) { return cub::DeviceSelect::Flagged(t, b, counting, alive, ids0, d_num, F, st); });
+            A = read_back(d_num, 1, st)[0];
         } else {
             A = C;
         }
     }
-    counters(h);
+    h = read_back(cnt, C_COUNT, st);
     R.merged_vertices = V - (int64_t)h[C_HEADS];
     R.nonfinite_faces = (int64_t)h[C_NONFINITE];
     R.degenerate_faces = (int64_t)h[C_DEGENERATE];
@@ -578,29 +545,30 @@ void mesh_clean(const float* verts, int64_t V64, const int32_t* faces, int64_t F
 
     // working faces: the A survivors in input order, then at most A fill faces (a face borders at most one fillable
     // loop, and a loop gets at most one fill face per bordering face)
-    int32_t* W = sc.W.as<int32_t>(6 * (size_t)std::max(A, 1));
-    if (A > 0) P2S_LAUNCH(mc_build_work_kernel, grid(A), 256, 0, st, faces, rep, ids0, A, W);
+    int32_t* W = ws.get<int32_t>(6 * (size_t)std::max(A, 1));
+    if (A > 0) P2S_LAUNCH(mc_build_work_kernel, grid1d(A, 256), 256, 0, st, faces, rep, ids0, A, W);
 
     // 4.-5. classify, fill holes, classify again
-    Edges e = classify(W, A, st);
+    const size_t classify_slots = ws.mark();
+    Edges e = classify(ws, classify_slots, W, A, st);
     int n = A;
     if (e.boundary > 0) {
-        int32_t* deg = sc.deg.as<int32_t>(V);
-        uint32_t* nb = sc.nb.as<uint32_t>(2 * (size_t)V);
-        int32_t *nfill = sc.nfill.as<int32_t>(V), *foff = sc.foff.as<int32_t>(V);
+        int32_t* deg = ws.get<int32_t>(V);
+        uint32_t* nb = ws.get<uint32_t>(2 * (size_t)V);
+        int32_t *nfill = ws.get<int32_t>(V), *foff = ws.get<int32_t>(V);
         P2S_CUDA(cudaMemsetAsync(deg, 0, (size_t)V * sizeof(int32_t), st));
-        P2S_LAUNCH(mc_boundary_kernel, grid(e.R), 256, 0, st, W, e.he, e.rcnt, e.roff, e.R, deg, nb);
-        P2S_LAUNCH(mc_loop_count_kernel, grid(V), 256, 0, st, deg, nb, V, nfill);
-        cub_run([&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, nfill, foff, V, st); });
-        const int added = read1(foff + (V - 1), st) + read1(nfill + (V - 1), st);
+        P2S_LAUNCH(mc_boundary_kernel, grid1d(e.R, 256), 256, 0, st, W, e.he, e.rcnt, e.roff, e.R, deg, nb);
+        P2S_LAUNCH(mc_loop_count_kernel, grid1d(V, 256), 256, 0, st, deg, nb, V, nfill);
+        cub_run(ws, 1, [&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, nfill, foff, V, st); });
+        const int added = read_back(foff + (V - 1), 1, st)[0] + read_back(nfill + (V - 1), 1, st)[0];
         P2S_CHECK(added <= A, "internal error: more fill faces than faces");
         if (added > 0) {
-            P2S_LAUNCH(mc_fill_kernel, grid(V), 256, 0, st, deg, nb, V, foff, A, W, cnt);
+            P2S_LAUNCH(mc_fill_kernel, grid1d(V, 256), 256, 0, st, deg, nb, V, foff, A, W, cnt);
             n = A + added;
-            e = classify(W, n, st);
+            e = classify(ws, classify_slots, W, n, st);
         }
     }
-    counters(h);
+    h = read_back(cnt, C_COUNT, st);
     R.holes_filled = (int64_t)h[C_HOLES];
     R.faces_added = n - A;
     R.boundary_edges = e.boundary;
@@ -610,52 +578,52 @@ void mesh_clean(const float* verts, int64_t V64, const int32_t* faces, int64_t F
 
     // 6. orientation of every component over two-face edges, only when the winding is inconsistent
     if (e.inconsistent > 0) {
-        auto* par = sc.par.as<unsigned long long>(n);
-        uint8_t *has2 = sc.has2.as<uint8_t>(n), *parity = sc.parity.as<uint8_t>(n);
-        uint8_t *nonorient = sc.nonorient.as<uint8_t>(n), *flip = sc.flip.as<uint8_t>(n);
-        int32_t* root = sc.root.as<int32_t>(n);
+        auto* par = ws.get<unsigned long long>(n);
+        uint8_t *has2 = ws.get<uint8_t>(n), *parity = ws.get<uint8_t>(n);
+        uint8_t *nonorient = ws.get<uint8_t>(n), *flip = ws.get<uint8_t>(n);
+        int32_t* root = ws.get<int32_t>(n);
         P2S_CUDA(cudaMemsetAsync(has2, 0, n, st));
         P2S_CUDA(cudaMemsetAsync(nonorient, 0, n, st));
         P2S_CUDA(cudaMemsetAsync(flip, 0, n, st));
-        P2S_LAUNCH(mc_init_parent_kernel, grid(n), 256, 0, st, par, n);
-        P2S_LAUNCH(mc_union_kernel, grid(e.R), 256, 0, st, W, e.he, e.rcnt, e.roff, e.R, par, has2);
-        P2S_LAUNCH(mc_flatten_kernel, grid(n), 256, 0, st, par, n, root, parity);
-        P2S_LAUNCH(mc_orientable_kernel, grid(e.R), 256, 0, st, W, e.he, e.rcnt, e.roff, e.R, root, parity, nonorient);
+        P2S_LAUNCH(mc_init_parent_kernel, grid1d(n, 256), 256, 0, st, par, n);
+        P2S_LAUNCH(mc_union_kernel, grid1d(e.R, 256), 256, 0, st, W, e.he, e.rcnt, e.roff, e.R, par, has2);
+        P2S_LAUNCH(mc_flatten_kernel, grid1d(n, 256), 256, 0, st, par, n, root, parity);
+        P2S_LAUNCH(mc_orientable_kernel, grid1d(e.R, 256), 256, 0, st, W, e.he, e.rcnt, e.roff, e.R, root, parity, nonorient);
         // faces with a two-face edge, grouped by component (stable: ascending face index inside)
-        int32_t *sel = sc.sel.as<int32_t>(n), *sel_s = sc.sel_s.as<int32_t>(n);
-        cub_run([&](void* t, size_t& b) { return cub::DeviceSelect::Flagged(t, b, counting, has2, sel, d_num, n, st); });
-        const int m = read1(d_num, st);
-        int32_t *sroot = sc.selroot.as<int32_t>(m), *sroot_s = sc.selroot_s.as<int32_t>(m);
-        P2S_LAUNCH(mc_gather_kernel<int32_t>, grid(m), 256, 0, st, root, sel, m, sroot);
-        cub_run([&](void* t, size_t& b) { return cub::DeviceRadixSort::SortPairs(t, b, sroot, sroot_s, sel, sel_s, m, 0, 32, st); });
-        int32_t *segroot = sc.segroot.as<int32_t>(m), *segcnt = sc.segcnt.as<int32_t>(m), *segoff = sc.segoff.as<int32_t>(m);
-        cub_run([&](void* t, size_t& b) { return cub::DeviceRunLengthEncode::Encode(t, b, sroot_s, segroot, segcnt, d_num, m, st); });
-        const int nseg = read1(d_num, st);
-        cub_run([&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, segcnt, segoff, nseg, st); });
-        double* det = sc.det.as<double>(m);
-        double* segsum = sc.segsum.as<double>(nseg);
-        P2S_LAUNCH(mc_det_kernel, grid(m), 256, 0, st, verts, W, sel_s, m, parity, det);
+        int32_t *sel = ws.get<int32_t>(n), *sel_s = ws.get<int32_t>(n);
+        cub_run(ws, 1, [&](void* t, size_t& b) { return cub::DeviceSelect::Flagged(t, b, counting, has2, sel, d_num, n, st); });
+        const int m = read_back(d_num, 1, st)[0];
+        int32_t *sroot = ws.get<int32_t>(m), *sroot_s = ws.get<int32_t>(m);
+        P2S_LAUNCH(mc_gather_kernel<int32_t>, grid1d(m, 256), 256, 0, st, root, sel, m, sroot);
+        cub_run(ws, 1, [&](void* t, size_t& b) { return cub::DeviceRadixSort::SortPairs(t, b, sroot, sroot_s, sel, sel_s, m, 0, 32, st); });
+        int32_t *segroot = ws.get<int32_t>(m), *segcnt = ws.get<int32_t>(m), *segoff = ws.get<int32_t>(m);
+        cub_run(ws, 1, [&](void* t, size_t& b) { return cub::DeviceRunLengthEncode::Encode(t, b, sroot_s, segroot, segcnt, d_num, m, st); });
+        const int nseg = read_back(d_num, 1, st)[0];
+        cub_run(ws, 1, [&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, segcnt, segoff, nseg, st); });
+        double* det = ws.get<double>(m);
+        double* segsum = ws.get<double>(nseg);
+        P2S_LAUNCH(mc_det_kernel, grid1d(m, 256), 256, 0, st, verts, W, sel_s, m, parity, det);
         P2S_CHECK(nseg > 0, "internal error: inconsistent winding without a two-face edge");
         P2S_LAUNCH(mc_segment_sum_kernel, nseg, kSumThreads, 0, st, det, segoff, segcnt, 0, segsum);
-        P2S_LAUNCH(mc_component_kernel, grid(nseg), 256, 0, st, segroot, segsum, nseg, nonorient, flip, cnt);
-        P2S_LAUNCH(mc_reverse_kernel, grid(n), 256, 0, st, W, n, has2, root, parity, nonorient, flip, cnt);
-        counters(h);
+        P2S_LAUNCH(mc_component_kernel, grid1d(nseg, 256), 256, 0, st, segroot, segsum, nseg, nonorient, flip, cnt);
+        P2S_LAUNCH(mc_reverse_kernel, grid1d(n, 256), 256, 0, st, W, n, has2, root, parity, nonorient, flip, cnt);
+        h = read_back(cnt, C_COUNT, st);
         R.components = nseg;
         R.nonorientable_components = (int64_t)h[C_NONORIENT];
         R.faces_reversed = (int64_t)h[C_REVERSED];
-        e = classify(W, n, st);
+        e = classify(ws, classify_slots, W, n, st);
     }
     R.watertight = e.boundary == 0 && e.nonmanifold == 0;
     R.winding_consistent = e.inconsistent == 0;
 
     // 7. drop unreferenced vertices; signed volume of the output
-    int32_t *used = sc.used.as<int32_t>(V), *newidx = sc.newidx.as<int32_t>(V);
+    int32_t *used = ws.get<int32_t>(V), *newidx = ws.get<int32_t>(V);
     int vout = 0;
     if (V > 0) {
         P2S_CUDA(cudaMemsetAsync(used, 0, (size_t)V * sizeof(int32_t), st));
-        if (n > 0) P2S_LAUNCH(mc_mark_used_kernel, grid(3 * (int64_t)n), 256, 0, st, W, 3 * n, used);
-        cub_run([&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, used, newidx, V, st); });
-        vout = read1(newidx + (V - 1), st) + read1(used + (V - 1), st);
+        if (n > 0) P2S_LAUNCH(mc_mark_used_kernel, grid1d(3 * (int64_t)n, 256), 256, 0, st, W, 3 * n, used);
+        cub_run(ws, 1, [&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, used, newidx, V, st); });
+        vout = read_back(newidx + (V - 1), 1, st)[0] + read_back(used + (V - 1), 1, st)[0];
     }
     R.vertices_out = vout;
     R.faces_out = n;
@@ -664,10 +632,10 @@ void mesh_clean(const float* verts, int64_t V64, const int32_t* faces, int64_t F
     P2S_CHECK(n <= fcap, "fcap too small for the cleaned mesh (fcap >= 2 F always suffices)");
     P2S_CHECK((verts_out || vout == 0) && (faces_out || n == 0), "null output");
     if (n > 0) {
-        double* det = sc.det.as<double>(n);
-        P2S_LAUNCH(mc_det_kernel, grid(n), 256, 0, st, verts, W, nullptr, n, nullptr, det);
-        R.volume = fixed_sum(det, n, st) / 6.0;
-        P2S_LAUNCH(mc_emit_kernel, grid(std::max(V, 3 * n)), 256, 0, st, verts, V, used, newidx, W, 3 * n, verts_out,
+        double* det = ws.get<double>(n);
+        P2S_LAUNCH(mc_det_kernel, grid1d(n, 256), 256, 0, st, verts, W, nullptr, n, nullptr, det);
+        R.volume = fixed_sum(ws, det, n, st) / 6.0;
+        P2S_LAUNCH(mc_emit_kernel, grid1d(std::max(V, 3 * n), 256), 256, 0, st, verts, V, used, newidx, W, 3 * n, verts_out,
                    faces_out);
         P2S_CUDA(cudaStreamSynchronize(st));
     }

@@ -269,28 +269,19 @@ mesh_closest_finalize_kernel(const double* __restrict__ part_d2, const int32_t* 
     closest[3 * i] = (float)cp[0]; closest[3 * i + 1] = (float)cp[1]; closest[3 * i + 2] = (float)cp[2];
 }
 
-struct Scratch {
-    DevBuf flags, d2, face, wind;
-};
-Scratch& scratch() {
-    static thread_local Scratch s;
-    return s;
-}
-
 // kSigned: signed distance (+ winding); else unsigned distance (+ closest point)
 template <bool kSigned>
 void mesh_query(const float* verts, int64_t V, const int32_t* faces, int64_t F, const float* query, int64_t Q,
                 float* dist, int32_t* closest_face, float* winding, float* closest, cudaStream_t st) {
     P2S_CHECK(V > 0 && F > 0, "empty mesh");
     P2S_CHECK(V <= INT32_MAX && F <= INT32_MAX / 3, "mesh too large for int32 indices");
-    auto& sc = scratch();
-    unsigned* flags = sc.flags.as<unsigned>(2);   // [0] out-of-range face indices, [1] max |vertex coordinate| (bits)
+    static thread_local std::vector<Workspace> t_ws;   // one per instantiation: signed distance, closest point
+    Workspace& ws = for_device(t_ws).begin(st);
+    unsigned* flags = ws.get<unsigned>(2);   // [0] out-of-range face indices, [1] max |vertex coordinate| (bits)
     P2S_CUDA(cudaMemsetAsync(flags, 0, 2 * sizeof(unsigned), st));
     const int64_t n = 3 * std::max(V, F);
     P2S_LAUNCH(mesh_check_kernel, (unsigned)cdiv(n, 256), 256, 0, st, verts, V, faces, F, flags);
-    unsigned h[2];
-    P2S_CUDA(cudaMemcpyAsync(h, flags, sizeof(h), cudaMemcpyDeviceToHost, st));
-    P2S_CUDA(cudaStreamSynchronize(st));
+    const std::vector<unsigned> h = read_back(flags, 2, st);
     P2S_CHECK(h[0] == 0, "face index outside [0, V)");
     float vmax;
     memcpy(&vmax, &h[1], 4);
@@ -300,9 +291,9 @@ void mesh_query(const float* verts, int64_t V, const int32_t* faces, int64_t F, 
     const int64_t slab_len = std::max<int64_t>(kTile, cdiv(cdiv(F, kMaxSlabs), kTile) * kTile);
     const int slabs = (int)cdiv(F, slab_len);
     const int64_t qc = std::min(Q, kChunk);
-    double* d2 = sc.d2.as<double>((size_t)slabs * qc);
-    int32_t* fc = sc.face.as<int32_t>((size_t)slabs * qc);
-    double* wn = kSigned ? sc.wind.as<double>((size_t)slabs * qc) : nullptr;
+    double* d2 = ws.get<double>(slabs * qc);
+    int32_t* fc = ws.get<int32_t>(slabs * qc);
+    double* wn = kSigned ? ws.get<double>(slabs * qc) : nullptr;
     for (int64_t q0 = 0; q0 < Q; q0 += kChunk) {
         const int64_t nq = std::min(kChunk, Q - q0);
         P2S_LAUNCH(meshsdf_slab_kernel<kSigned>, dim3((unsigned)cdiv(nq, kThreads), (unsigned)slabs), kThreads, 0, st, verts,

@@ -631,10 +631,7 @@ void tc_build(Model& m) {
         s.b3 = f.conv3.b;
     };
     fc_tc_init();
-    {
-        const char* e = getenv("P2S_FC_FP32");
-        t->fc_on_tc = !(e && e[0] == '1');
-    }
+    t->fc_on_tc = !env_flag("P2S_FC_FP32");
     auto mk_fc = [&](const Layer& L) {
         TcFc f;
         f.L = &L;
@@ -808,8 +805,7 @@ static void forward_tc_core(Model& m, const float* patch, const float* sub, cons
 // accurate recompute used for the guard band: split-precision tensor-core path (default) or the fp32 FMA path
 // (environment P2S_GUARD_FP32=1)
 void forward_guard(Model& m, const float* patch, const float* sub, const float* query, int64_t B, float* logits, cudaStream_t st) {
-    static int use_fp32 = -1;
-    if (use_fp32 < 0) { const char* e = getenv("P2S_GUARD_FP32"); use_fp32 = (e && e[0] == '1') ? 1 : 0; }
+    static const bool use_fp32 = env_flag("P2S_GUARD_FP32");
     if (use_fp32) forward_fp32(m, patch, sub, query, B, logits, st);
     else forward_tc_core(m, patch, sub, query, B, logits, st, true);
 }

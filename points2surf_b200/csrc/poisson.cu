@@ -565,37 +565,6 @@ poisson_output_kernel(const double* __restrict__ chi, const double* __restrict__
 }
 
 // ---- host side
-// grow-only device buffers, handed out in call order: the same sequence of requests reuses the same buffers
-thread_local std::vector<DevBuf> t_bufs;
-thread_local DevBuf t_cub;
-
-struct Pool {
-    size_t next = 0;
-    template <class T>
-    T* get(int64_t count) {
-        if (next == t_bufs.size()) t_bufs.emplace_back();
-        return reinterpret_cast<T*>(t_bufs[next++].get((size_t)std::max<int64_t>(count, 1) * sizeof(T)));
-    }
-};
-
-unsigned grid(int64_t n) { return (unsigned)cdiv(std::max<int64_t>(n, 1), 256); }
-
-template <class Fn>
-void cub_run(Fn fn) {
-    size_t bytes = 0;
-    P2S_CUDA(fn(nullptr, bytes));
-    P2S_CUDA(fn(t_cub.get(std::max<size_t>(bytes, 16)), bytes));
-    g_launches.fetch_add(1, std::memory_order_relaxed);   // counts the CUB call once, whatever it launches
-}
-
-template <class T>
-T read1(const T* dev, cudaStream_t st) {
-    T h;
-    P2S_CUDA(cudaMemcpyAsync(&h, dev, sizeof(T), cudaMemcpyDeviceToHost, st));
-    P2S_CUDA(cudaStreamSynchronize(st));
-    return h;
-}
-
 struct Level {
     int n = 0;
     int64_t nn = 0, ncell = 0;
@@ -621,7 +590,7 @@ struct Solver {
     }
     template <int OP>
     void level_op(const Level& L, const double* x, const double* b, double* out) {
-        P2S_LAUNCH(poisson_level_kernel<OP>, grid(L.nn), 256, 0, st, L.view(), x, b, out);
+        P2S_LAUNCH(poisson_level_kernel<OP>, grid1d(L.nn, 256), 256, 0, st, L.view(), x, b, out);
     }
     // x = V-cycle(b) on level l
     void vcycle(int l, const double* b, double* x) {
@@ -632,16 +601,16 @@ struct Solver {
         }
         // 2 nu - 1 ping-pong swaps follow the first sweep, so starting in t leaves the result in x
         double *cur = L.t, *oth = x;
-        P2S_LAUNCH(poisson_jacobi0_kernel, grid(L.nn), 256, 0, st, L.invD, b, L.nn, cur);
+        P2S_LAUNCH(poisson_jacobi0_kernel, grid1d(L.nn, 256), 256, 0, st, L.invD, b, L.nn, cur);
         for (int s = 1; s < nu; ++s) {
             level_op<OP_JACOBI>(L, cur, b, oth);
             std::swap(cur, oth);
         }
         level_op<OP_RESIDUAL>(L, cur, b, L.r);
         const Level& C = lv[l - 1];
-        P2S_LAUNCH(poisson_restrict_kernel, grid(C.nn), 256, 0, st, C.n, L.r, C.b);
+        P2S_LAUNCH(poisson_restrict_kernel, grid1d(C.nn, 256), 256, 0, st, C.n, L.r, C.b);
         vcycle(l - 1, C.b, C.x);
-        P2S_LAUNCH(poisson_prolong_add_kernel, grid(L.nn), 256, 0, st, C.n, C.x, cur);
+        P2S_LAUNCH(poisson_prolong_add_kernel, grid1d(L.nn, 256), 256, 0, st, C.n, C.x, cur);
         for (int s = 0; s < nu; ++s) {
             level_op<OP_JACOBI>(L, cur, b, oth);
             std::swap(cur, oth);
@@ -675,17 +644,15 @@ void poisson_solve(const float* pts, const float* nrm, int64_t N, const p2s_pois
         ~EvGuard() { for (int k = 0; k < 5; ++k) cudaEventDestroy(e[k]); }
     } evg{ev};
     P2S_CUDA(cudaEventRecord(ev[0], st));
-    Pool pool;
+    static thread_local std::vector<Workspace> t_ws;
+    Workspace& ws = for_device(t_ws).begin(st);
 
     // 1. bounding box and input checks
-    float* box = pool.get<float>(kRedBlocks * 6);
-    int64_t* counts = pool.get<int64_t>(kRedBlocks * 2);
+    float* box = ws.get<float>(kRedBlocks * 6);
+    int64_t* counts = ws.get<int64_t>(kRedBlocks * 2);
     P2S_LAUNCH(poisson_bbox_kernel, kRedBlocks, kRedThreads, 0, st, pts, nrm, N, box, counts);
-    std::vector<float> hbox(kRedBlocks * 6);
-    std::vector<int64_t> hcnt(kRedBlocks * 2);
-    P2S_CUDA(cudaMemcpyAsync(hbox.data(), box, hbox.size() * sizeof(float), cudaMemcpyDeviceToHost, st));
-    P2S_CUDA(cudaMemcpyAsync(hcnt.data(), counts, hcnt.size() * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
-    P2S_CUDA(cudaStreamSynchronize(st));
+    const std::vector<float> hbox = read_back(box, kRedBlocks * 6, st);
+    const std::vector<int64_t> hcnt = read_back(counts, kRedBlocks * 2, st);
     float lo[3] = {INFINITY, INFINITY, INFINITY}, hi[3] = {-INFINITY, -INFINITY, -INFINITY};
     int64_t bad = 0, dropped = 0;
     for (int b = 0; b < kRedBlocks; ++b) {
@@ -712,30 +679,30 @@ void poisson_solve(const float* pts, const float* nrm, int64_t N, const p2s_pois
     rep->dropped_points = dropped;
 
     // 2. sort by the Morton key of the finest cell
-    uint32_t* key_in = pool.get<uint32_t>(N);
-    uint32_t* key = pool.get<uint32_t>(N);
-    int32_t* idx_in = pool.get<int32_t>(N);
-    int32_t* order = pool.get<int32_t>(N);
-    P2S_LAUNCH(poisson_key_kernel, grid(N), 256, 0, st, pts, nrm, N, f, d, key_in, idx_in);
-    cub_run([&](void* t, size_t& b) {
+    uint32_t* key_in = ws.get<uint32_t>(N);
+    uint32_t* key = ws.get<uint32_t>(N);
+    int32_t* idx_in = ws.get<int32_t>(N);
+    int32_t* order = ws.get<int32_t>(N);
+    P2S_LAUNCH(poisson_key_kernel, grid1d(N, 256), 256, 0, st, pts, nrm, N, f, d, key_in, idx_in);
+    cub_run(ws, 1, [&](void* t, size_t& b) {
         return cub::DeviceRadixSort::SortPairs(t, b, key_in, key, idx_in, order, (int)N, 0, 3 * d + 1, st);
     });
-    double* g = pool.get<double>(3 * Nk);
-    double* un = pool.get<double>(3 * Nk);
-    P2S_LAUNCH(poisson_gather_kernel, grid(Nk), 256, 0, st, order, Nk, pts, nrm, f, g, un);
+    double* g = ws.get<double>(3 * Nk);
+    double* un = ws.get<double>(3 * Nk);
+    P2S_LAUNCH(poisson_gather_kernel, grid1d(Nk, 256), 256, 0, st, order, Nk, pts, nrm, f, g, un);
 
     // 3. area weights from the point count of the depth d-2 cell
-    int32_t* d_num = pool.get<int32_t>(1);
-    uint32_t* skey = pool.get<uint32_t>(Nk);
-    uint32_t* ukey_dens = pool.get<uint32_t>(Nk);
-    int32_t* cnt_dens = pool.get<int32_t>(Nk);
-    double* area = pool.get<double>(Nk);
-    P2S_LAUNCH(poisson_shift_kernel, grid(Nk), 256, 0, st, key, Nk, 6, skey);
-    cub_run([&](void* t, size_t& b) {
+    int32_t* d_num = ws.get<int32_t>(1);
+    uint32_t* skey = ws.get<uint32_t>(Nk);
+    uint32_t* ukey_dens = ws.get<uint32_t>(Nk);
+    int32_t* cnt_dens = ws.get<int32_t>(Nk);
+    double* area = ws.get<double>(Nk);
+    P2S_LAUNCH(poisson_shift_kernel, grid1d(Nk, 256), 256, 0, st, key, Nk, 6, skey);
+    cub_run(ws, 1, [&](void* t, size_t& b) {
         return cub::DeviceRunLengthEncode::Encode(t, b, skey, ukey_dens, cnt_dens, d_num, (int)Nk, st);
     });
-    const int ndens = read1(d_num, st);
-    P2S_LAUNCH(poisson_area_kernel, grid(Nk), 256, 0, st, key, Nk, 6, ukey_dens, cnt_dens, ndens, 16.0 / ((double)n * n),
+    const int ndens = read_back(d_num, 1, st)[0];
+    P2S_LAUNCH(poisson_area_kernel, grid1d(Nk, 256), 256, 0, st, key, Nk, 6, ukey_dens, cnt_dens, ndens, 16.0 / ((double)n * n),
                area);
 
     // 4. cells of every level
@@ -744,11 +711,11 @@ void poisson_solve(const float* pts, const float* nrm, int64_t N, const p2s_pois
     sv.depth = d;
     sv.nu = cfg.iters;
     sv.lv.resize(d + 1);
-    sv.partial = pool.get<double>(kRedBlocks);
-    sv.sc = pool.get<double>(SC_COUNT);
+    sv.partial = ws.get<double>(kRedBlocks);
+    sv.sc = ws.get<double>(SC_COUNT);
     const double alpha = (double)cfg.point_weight * (double)n;
-    int32_t* cell_cnt = pool.get<int32_t>(Nk);
-    int32_t* cell_start = pool.get<int32_t>(Nk);
+    int32_t* cell_cnt = ws.get<int32_t>(Nk);
+    int32_t* cell_start = ws.get<int32_t>(Nk);
     double* W = nullptr;
     for (int l = d; l >= kCoarseDepth; --l) {
         Level& L = sv.lv[l];
@@ -756,27 +723,27 @@ void poisson_solve(const float* pts, const float* nrm, int64_t N, const p2s_pois
         L.nn = (int64_t)(L.n + 1) * (L.n + 1) * (L.n + 1);
         const int64_t ncells_dense = (int64_t)L.n * L.n * L.n;
         if (l == d) {
-            L.ukey = pool.get<uint32_t>(Nk);
-            cub_run([&](void* t, size_t& b) {
+            L.ukey = ws.get<uint32_t>(Nk);
+            cub_run(ws, 1, [&](void* t, size_t& b) {
                 return cub::DeviceRunLengthEncode::Encode(t, b, key, L.ukey, cell_cnt, d_num, (int)Nk, st);
             });
         } else {
             const Level& F = sv.lv[l + 1];
-            L.ukey = pool.get<uint32_t>(F.ncell);
-            P2S_LAUNCH(poisson_shift_kernel, grid(F.ncell), 256, 0, st, F.ukey, F.ncell, 3, skey);
-            cub_run([&](void* t, size_t& b) {
+            L.ukey = ws.get<uint32_t>(F.ncell);
+            P2S_LAUNCH(poisson_shift_kernel, grid1d(F.ncell, 256), 256, 0, st, F.ukey, F.ncell, 3, skey);
+            cub_run(ws, 1, [&](void* t, size_t& b) {
                 return cub::DeviceRunLengthEncode::Encode(t, b, skey, L.ukey, cell_cnt, d_num, (int)F.ncell, st);
             });
         }
-        L.ncell = read1(d_num, st);
-        L.slot = pool.get<int32_t>(ncells_dense);
-        L.S = pool.get<double>(L.ncell * 36);
+        L.ncell = read_back(d_num, 1, st)[0];
+        L.slot = ws.get<int32_t>(ncells_dense);
+        L.S = ws.get<double>(L.ncell * 36);
         P2S_CUDA(cudaMemsetAsync(L.slot, 0xff, (size_t)ncells_dense * sizeof(int32_t), st));
         if (l == d) {
-            cub_run([&](void* t, size_t& b) {
+            cub_run(ws, 1, [&](void* t, size_t& b) {
                 return cub::DeviceScan::ExclusiveSum(t, b, cell_cnt, cell_start, (int)L.ncell, st);
             });
-            W = pool.get<double>(L.ncell * 24);
+            W = ws.get<double>(L.ncell * 24);
             P2S_LAUNCH(poisson_fine_cells_kernel, (unsigned)cdiv(L.ncell, 128), 128, 0, st, L.ukey, cell_start, cell_cnt,
                        (int)L.ncell, L.n, g, un, area, Nk, alpha, L.slot, L.S, W);
             rep->occupied_cells = L.ncell;
@@ -784,35 +751,35 @@ void poisson_solve(const float* pts, const float* nrm, int64_t N, const p2s_pois
             P2S_LAUNCH(poisson_coarse_cells_kernel, (unsigned)cdiv(L.ncell, 128), 128, 0, st, L.ukey, (int)L.ncell, L.n,
                        sv.lv[l + 1].view(), L.slot, L.S);
         }
-        L.invD = pool.get<double>(L.nn);
-        P2S_LAUNCH(poisson_invdiag_kernel, grid(L.nn), 256, 0, st, L.view(), L.invD);
-        L.t = pool.get<double>(L.nn);
-        L.r = pool.get<double>(L.nn);
+        L.invD = ws.get<double>(L.nn);
+        P2S_LAUNCH(poisson_invdiag_kernel, grid1d(L.nn, 256), 256, 0, st, L.view(), L.invD);
+        L.t = ws.get<double>(L.nn);
+        L.r = ws.get<double>(L.nn);
         if (l < d) {
-            L.x = pool.get<double>(L.nn);
-            L.b = pool.get<double>(L.nn);
+            L.x = ws.get<double>(L.nn);
+            L.b = ws.get<double>(L.nn);
         }
     }
     P2S_CUDA(cudaEventRecord(ev[1], st));
 
     // 5. right-hand side
     const Level& Fl = sv.lv[d];
-    double* V = pool.get<double>(3 * nn);
-    double* B = pool.get<double>(nn);
-    P2S_LAUNCH(poisson_vfield_kernel, grid(nn), 256, 0, st, n, Fl.slot, W, V);
-    P2S_LAUNCH(poisson_rhs_kernel, grid(nn), 256, 0, st, n, V, B);
+    double* V = ws.get<double>(3 * nn);
+    double* B = ws.get<double>(nn);
+    P2S_LAUNCH(poisson_vfield_kernel, grid1d(nn, 256), 256, 0, st, n, Fl.slot, W, V);
+    P2S_LAUNCH(poisson_rhs_kernel, grid1d(nn, 256), 256, 0, st, n, V, B);
     P2S_CUDA(cudaEventRecord(ev[2], st));
 
     // 6. MG-preconditioned CG from chi = 0
-    double* X = pool.get<double>(nn);
-    double* Rr = pool.get<double>(nn);
-    double* Z = pool.get<double>(nn);
-    double* P = pool.get<double>(nn);
-    double* Q = pool.get<double>(nn);
+    double* X = ws.get<double>(nn);
+    double* Rr = ws.get<double>(nn);
+    double* Z = ws.get<double>(nn);
+    double* P = ws.get<double>(nn);
+    double* Q = ws.get<double>(nn);
     P2S_CUDA(cudaMemsetAsync(X, 0, (size_t)nn * sizeof(double), st));
     P2S_CUDA(cudaMemcpyAsync(Rr, B, (size_t)nn * sizeof(double), cudaMemcpyDeviceToDevice, st));
     sv.dot(B, B, nn, SC_RR);
-    const double bb = read1(sv.sc + SC_RR, st);
+    const double bb = read_back(sv.sc + SC_RR, 1, st)[0];
     int it = 0;
     double residual = 0.0;
     if (bb > 0.0) {
@@ -825,10 +792,10 @@ void poisson_solve(const float* pts, const float* nrm, int64_t N, const p2s_pois
         while (it < kMaxIters) {
             sv.level_op<OP_APPLY>(Fl, P, nullptr, Q);
             sv.dot(P, Q, nn, SC_PQ);
-            P2S_LAUNCH(poisson_cg_x_kernel, grid(nn), 256, 0, st, sv.sc, rz, P, Q, X, Rr, nn);
+            P2S_LAUNCH(poisson_cg_x_kernel, grid1d(nn, 256), 256, 0, st, sv.sc, rz, P, Q, X, Rr, nn);
             sv.dot(Rr, Rr, nn, SC_RR);
             ++it;
-            const double rel = std::sqrt(read1(sv.sc + SC_RR, st) / bb);
+            const double rel = std::sqrt(read_back(sv.sc + SC_RR, 1, st)[0] / bb);
             if (!(rel > kRelTol)) break;   // converged (or not a number: stop)
             if (rel < best) {
                 best = rel;
@@ -838,27 +805,25 @@ void poisson_solve(const float* pts, const float* nrm, int64_t N, const p2s_pois
             }
             sv.vcycle(d, Rr, Z);
             sv.dot(Rr, Z, nn, rz ^ 1);
-            P2S_LAUNCH(poisson_cg_p_kernel, grid(nn), 256, 0, st, sv.sc, rz, rz ^ 1, Z, P, nn);
+            P2S_LAUNCH(poisson_cg_p_kernel, grid1d(nn, 256), 256, 0, st, sv.sc, rz, rz ^ 1, Z, P, nn);
             rz ^= 1;
         }
         sv.level_op<OP_RESIDUAL>(Fl, X, B, Rr);   // report the true residual, not the recursive one
         sv.dot(Rr, Rr, nn, SC_RR);
-        residual = std::sqrt(read1(sv.sc + SC_RR, st) / bb);
+        residual = std::sqrt(read_back(sv.sc + SC_RR, 1, st)[0] / bb);
     }
     rep->iterations = it;
     rep->residual = residual;
     P2S_CUDA(cudaEventRecord(ev[3], st));
 
     // 7. iso-value and output
-    double* chi_p = pool.get<double>(Nk);
-    P2S_LAUNCH(poisson_point_chi_kernel, grid(Nk), 256, 0, st, g, Nk, n, X, chi_p);
+    double* chi_p = ws.get<double>(Nk);
+    P2S_LAUNCH(poisson_point_chi_kernel, grid1d(Nk, 256), 256, 0, st, g, Nk, n, X, chi_p);
     sv.dot(area, nullptr, Nk, SC_AREA);
     sv.dot(area, chi_p, Nk, SC_ACHI);
-    P2S_LAUNCH(poisson_output_kernel, grid(nn), 256, 0, st, X, sv.sc, nn, values);
+    P2S_LAUNCH(poisson_output_kernel, grid1d(nn, 256), 256, 0, st, X, sv.sc, nn, values);
     P2S_CUDA(cudaEventRecord(ev[4], st));
-    double s2[2];
-    P2S_CUDA(cudaMemcpyAsync(s2, sv.sc + SC_AREA, 2 * sizeof(double), cudaMemcpyDeviceToHost, st));
-    P2S_CUDA(cudaStreamSynchronize(st));
+    const std::vector<double> s2 = read_back(sv.sc + SC_AREA, 2, st);
     rep->iso = s2[1] / s2[0];
     for (int k = 0; k < 4; ++k) P2S_CUDA(cudaEventElapsedTime(&rep->stage_ms[k], ev[k], ev[k + 1]));
 }

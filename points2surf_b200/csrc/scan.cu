@@ -227,14 +227,6 @@ scan_emit_kernel(const double* __restrict__ poses, ScanParams P, const int32_t* 
     if (face_ids) face_ids[j] = face_ray[ri];
 }
 
-struct Scratch {
-    DevBuf flags, ray_flag, rays, t, face, hit, hitsel, cub, num;
-};
-Scratch& scratch() {
-    static thread_local Scratch s;
-    return s;
-}
-
 }  // namespace
 
 void range_scan(const float* verts, int64_t V, const int32_t* faces, int64_t F, const double* poses, int64_t S,
@@ -252,15 +244,14 @@ void range_scan(const float* verts, int64_t V, const int32_t* faces, int64_t F, 
     P2S_CHECK(cfg.first_scan >= 0, "first_scan must be >= 0");
     const int64_t npix = (int64_t)cfg.res_x * cfg.res_y;
     P2S_CHECK(npix <= INT32_MAX && S * npix <= INT32_MAX, "too many rays for one call (S * res_x * res_y >= 2^31)");
-    auto& sc = scratch();
-    unsigned* flags = sc.flags.as<unsigned>(7);
+    static thread_local std::vector<Workspace> t_ws;
+    Workspace& ws = for_device(t_ws).begin(st);
+    unsigned* flags = ws.get<unsigned>(7);
     unsigned init[7] = {0u, ~0u, ~0u, ~0u, 0u, 0u, 0u};
     P2S_CUDA(cudaMemcpyAsync(flags, init, sizeof(init), cudaMemcpyHostToDevice, st));
     const int64_t nchk = std::max(3 * F, V);
     P2S_LAUNCH(scan_check_kernel, (unsigned)cdiv(nchk, 256), 256, 0, st, verts, V, faces, F, flags);
-    unsigned h[7];
-    P2S_CUDA(cudaMemcpyAsync(h, flags, sizeof(h), cudaMemcpyDeviceToHost, st));
-    P2S_CUDA(cudaStreamSynchronize(st));
+    const std::vector<unsigned> h = read_back(flags, 7, st);
     P2S_CHECK(h[0] == 0, "face index outside [0, V)");
     ScanParams P;
     P.res_x = cfg.res_x; P.res_y = cfg.res_y; P.npix = (int)npix; P.first_scan = cfg.first_scan;
@@ -283,32 +274,22 @@ void range_scan(const float* verts, int64_t V, const int32_t* faces, int64_t F, 
     const int nrays = (int)(S * npix);
 
     cub::CountingInputIterator<int32_t> counting(0);
-    size_t cub_bytes = 0;
-    P2S_CUDA(cub::DeviceSelect::Flagged(nullptr, cub_bytes, counting, (uint8_t*)nullptr, (int32_t*)nullptr, (int*)nullptr,
-                                        nrays, st));
-    void* cub_tmp = sc.cub.get(cub_bytes);
-    int* d_num = sc.num.as<int>(1);
-    uint8_t* ray_flag = sc.ray_flag.as<uint8_t>((size_t)nrays);
-    int32_t* rays = sc.rays.as<int32_t>((size_t)nrays);
+    int* d_num = ws.get<int>(1);
+    uint8_t* ray_flag = ws.get<uint8_t>(nrays);
+    int32_t* rays = ws.get<int32_t>(nrays);
     P2S_LAUNCH(scan_cull_kernel, (unsigned)cdiv(nrays, 256), 256, 0, st, poses, (int64_t)nrays, P, ray_flag);
-    P2S_CUDA(cub::DeviceSelect::Flagged(cub_tmp, cub_bytes, counting, ray_flag, rays, d_num, nrays, st));
-    g_launches.fetch_add(2, std::memory_order_relaxed);  // cub: scan + select kernels
-    int n = 0;
-    P2S_CUDA(cudaMemcpyAsync(&n, d_num, sizeof(int), cudaMemcpyDeviceToHost, st));
-    P2S_CUDA(cudaStreamSynchronize(st));
+    cub_run(ws, 2, [&](void* t, size_t& b) { return cub::DeviceSelect::Flagged(t, b, counting, ray_flag, rays, d_num, nrays, st); });
+    const int n = read_back(d_num, 1, st)[0];
     if (n == 0) return;
 
-    double* t_ray = sc.t.as<double>((size_t)n);
-    int32_t* face_ray = sc.face.as<int32_t>((size_t)n);
-    uint8_t* hit = sc.hit.as<uint8_t>((size_t)n);
-    int32_t* hitsel = sc.hitsel.as<int32_t>((size_t)n);
+    double* t_ray = ws.get<double>(n);
+    int32_t* face_ray = ws.get<int32_t>(n);
+    uint8_t* hit = ws.get<uint8_t>(n);
+    int32_t* hitsel = ws.get<int32_t>(n);
     P2S_LAUNCH(scan_cast_kernel, (unsigned)cdiv(n, kThreads), kThreads, 0, st, verts, faces, F, poses, P, rays, n, t_ray,
                face_ray, hit);
-    P2S_CUDA(cub::DeviceSelect::Flagged(cub_tmp, cub_bytes, counting, hit, hitsel, d_num, n, st));
-    g_launches.fetch_add(2, std::memory_order_relaxed);
-    int H = 0;
-    P2S_CUDA(cudaMemcpyAsync(&H, d_num, sizeof(int), cudaMemcpyDeviceToHost, st));
-    P2S_CUDA(cudaStreamSynchronize(st));
+    cub_run(ws, 2, [&](void* t, size_t& b) { return cub::DeviceSelect::Flagged(t, b, counting, hit, hitsel, d_num, n, st); });
+    const int H = read_back(d_num, 1, st)[0];
     *total_host = H;
     if (H == 0) return;
     P2S_CHECK(cap == 0 || pts_noisy, "null output with cap > 0");

@@ -401,17 +401,6 @@ __global__ void center_kernel(const float* __restrict__ in, const float* __restr
     out[e] = in[e] - q[b * 3 + e % 3];
 }
 
-int sm_count() {
-    static int n = 0;
-    if (!n) {
-        int dev = 0;
-        cudaGetDevice(&dev);
-        cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-        if (n <= 0) n = 132;
-    }
-    return n;
-}
-
 }  // namespace
 
 // ---------------------------------------------------------------------------------------------- host launchers

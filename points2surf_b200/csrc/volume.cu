@@ -579,8 +579,6 @@ __global__ void finalize_kernel(float* __restrict__ vol, const uint8_t* __restri
     vol[v] = x;
 }
 
-thread_local DevBuf t_vol_ws;
-
 }  // namespace
 
 void sdf_from_logits(const float* logits, const float* radius, int64_t B, float* sdf, cudaStream_t st) {
@@ -602,19 +600,15 @@ void sdf_to_volume(const int32_t* lin_idx, const float* sdf, int64_t Q, int res,
     pp.maxIters = 64 * res;
     const int numTiles = pp.ntx * pp.nty * pp.ntz;
     const size_t nt4 = ((size_t)numTiles + 3) & ~(size_t)3;
-    size_t off = (sizeof(Ctrl) + 255) & ~(size_t)255;
-    const size_t off_A = off; off += (V + 255) & ~(size_t)255;
-    const size_t off_B = off; off += (V + 255) & ~(size_t)255;
-    const size_t off_lists = off; off += 3 * nt4 * sizeof(int);
-    const size_t off_vz = off; off += nt4 * sizeof(int);
-    const size_t off_flags = off; off += 2 * nt4;
-    uint8_t* base = (uint8_t*)t_vol_ws.get(off);
-    Ctrl* ctrl = (Ctrl*)base;
+    static thread_local std::vector<Workspace> t_ws;
+    Workspace& ws = for_device(t_ws).begin(st);
+    Ctrl* ctrl = ws.get<Ctrl>(1);
     pp.ctrl = ctrl;
-    pp.buf[0] = base + off_A; pp.buf[1] = base + off_B;
-    for (int i = 0; i < 3; ++i) pp.list[i] = (int*)(base + off_lists) + (size_t)i * nt4;
-    pp.voteZeros = (int*)(base + off_vz);
-    pp.flags[0] = base + off_flags; pp.flags[1] = base + off_flags + nt4;
+    pp.buf[0] = ws.get<uint8_t>(V); pp.buf[1] = ws.get<uint8_t>(V);
+    int* lists = ws.get<int>(3 * nt4);
+    for (int i = 0; i < 3; ++i) pp.list[i] = lists + (size_t)i * nt4;
+    pp.voteZeros = ws.get<int>(nt4);
+    pp.flags[0] = ws.get<uint8_t>(2 * nt4); pp.flags[1] = pp.flags[0] + nt4;
 
     P2S_CUDA(cudaMemsetAsync(ctrl, 0, sizeof(Ctrl), st));
     P2S_CUDA(cudaMemsetAsync(vol, 0, (size_t)V * sizeof(float), st));
@@ -633,17 +627,13 @@ void sdf_to_volume(const int32_t* lin_idx, const float* sdf, int64_t Q, int res,
     (void)Z0;
     pp.words = (res % 4 == 0) ? 1 : 0;       // aligned 32-bit row loads need word-aligned rows
     pp.fast = (pp.words && sigma <= 5) ? 1 : 0;   // packed biased-byte sums need 2 * sigma^3 <= 255
-    {
-        static int novec = -1;
-        if (novec < 0) { const char* e = getenv("P2S_VOL_NOVEC"); novec = (e && e[0] == '1') ? 1 : 0; }
-        pp.vec = (sigma == 5 && res % 32 == 0 && !novec) ? 1 : 0;   // row-vector path: full tiles, 16-byte aligned rows
-    }
+    static const bool novec = env_flag("P2S_VOL_NOVEC");
+    pp.vec = (sigma == 5 && res % 32 == 0 && !novec) ? 1 : 0;   // row-vector path: full tiles, 16-byte aligned rows
     const size_t smem_generic = (size_t)((X0 * Y0 * ZS + 15) & ~15) + (size_t)((X0 * Y0 * TZ + 15) & ~15) + (size_t)X0 * TY * TZ * 2;
     const size_t smem_fast = 4 * ((size_t)X0 * Y0 * (ZS / 4) + (size_t)TX * TY * 8 + (size_t)X0 * Y0 * 8 + (size_t)X0 * TY * 8);
     const size_t smem = pp.fast ? smem_fast : smem_generic;
-    int dev_id = 0, sms = 132, per_sm = 0;
-    P2S_CUDA(cudaGetDevice(&dev_id));
-    P2S_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev_id));
+    const int sms = sm_count();
+    int per_sm = 0;
     const bool s5 = pp.fast && sigma == 5;
     const void* kfn = s5 ? (const void*)propagate_kernel<true> : (const void*)propagate_kernel<false>;
     P2S_CUDA(cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
@@ -655,15 +645,12 @@ void sdf_to_volume(const int32_t* lin_idx, const float* sdf, int64_t Q, int res,
     P2S_CUDA(cudaLaunchCooperativeKernel(kfn, dim3(grid), dim3(kPropThreads), args, smem, st));
     g_launches.fetch_add(1, std::memory_order_relaxed);
     P2S_LAUNCH(finalize_kernel, blocks, 256, 0, st, vol, pp.buf[0], pp.buf[1], ctrl, V);
-    Ctrl h{};
-    P2S_CUDA(cudaMemcpyAsync(&h, ctrl, sizeof(Ctrl), cudaMemcpyDeviceToHost, st));
-    P2S_CUDA(cudaStreamSynchronize(st));
+    const Ctrl h = read_back(ctrl, 1, st)[0];
     P2S_CHECK(h.bad_index == 0, "voxel index outside [0, res^3): query points must lie in [-1, 1)^3 (the reference raises IndexError / wraps)");
     P2S_CHECK(h.error == 0, "sign propagation did not converge");
     if (iterations_host) *iterations_host = h.iters;
     {
-        static int stats = -1;
-        if (stats < 0) { const char* e = getenv("P2S_VOL_STATS"); stats = (e && e[0] == '1') ? 1 : 0; }
+        static const bool stats = env_flag("P2S_VOL_STATS");
         if (stats) fprintf(stderr, "p2s sign propagation: res %d, %d iterations, %llu tile evaluations over %d tiles (%.1f per tile; a full sweep per iteration would be %d), grid %u x %d threads, %zu B smem; kernel %.3f ms (block 0: %.3f ms inside grid.sync, first iteration %.3f ms)\n",
                            res, h.iters, h.visits, numTiles, (double)h.visits / numTiles, h.iters + 1, grid, kPropThreads, smem,
                            h.t_total * 1e-6, h.t_sync * 1e-6, h.t_first * 1e-6);
