@@ -144,13 +144,18 @@ def knn_bruteforce(pts, query_point, k):
 # --------------------------------------------------------------------------------------
 
 
-def sub_sample_probabilities(pts_ms, query_point_ms):
-    """source/base/utils.py:200-208 (float32 arithmetic like the reference)."""
+def sub_sample_weights(pts_ms, query_point_ms):
+    """The unnormalised weights of source/base/utils.py:200-207 (float32 arithmetic like the reference)."""
     query_pts = np.broadcast_to(query_point_ms, pts_ms.shape)
     dist = np.linalg.norm(query_pts - pts_ms, axis=1)
     dist_normalized = dist / np.max(dist)
     prob = 1.0 - 1.5 * dist_normalized
-    prob_clipped = np.clip(prob, 0.05, 1.0)
+    return np.clip(prob, 0.05, 1.0)
+
+
+def sub_sample_probabilities(pts_ms, query_point_ms):
+    """source/base/utils.py:200-208 (float32 arithmetic like the reference)."""
+    prob_clipped = sub_sample_weights(pts_ms, query_point_ms)
     return prob_clipped / np.sum(prob_clipped)
 
 

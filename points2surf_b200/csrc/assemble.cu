@@ -30,10 +30,20 @@ constexpr int kCapBig = 2048;   // kNN with 513..1536 neighbours (large_kNN: 120
 
 // ---- key helpers: non-negative doubles order like their bit patterns ----
 __device__ __forceinline__ unsigned long long dkey(double v) { return (unsigned long long)__double_as_longlong(v); }
-// level-0 bin: sign+exponent+4 mantissa bits, rebased so that 2^-100 .. 2^27 maps to 0..2047
+// level-0 bin: sign+exponent+4 mantissa bits, rebased so that 2^-100 .. 2^27 maps to 0..2047.  Keys below that range
+// share bin 0 and keys above it (2^27 and up, and the all-ones "no key") share bin 2047.
 __device__ __forceinline__ int bin0(unsigned long long key) {
     long long b = (long long)(key >> 48) - ((1023 - 100) << 4);
     return (int)(b < 0 ? 0 : (b > kBins - 1 ? kBins - 1 : b));
+}
+// refinement digit of `key` at level >= 1 inside level-0 bin b0: the next 11 bits below the ones the chain has fixed.  In an
+// interior bin the top 16 bits are fixed, so level l takes bits [48 - 11 l, 59 - 11 l).  A clamped bin fixes no bits: bin 0
+// holds keys < 2^62 and refines from bit 61 down, bin 2047 refines from bit 63 down.  Refinement therefore follows the
+// true key order in every bin, at 11 bits per level.  (The clock keys of the sub-samplers lie in 2^-24 .. 2^9 apart from an
+// exact zero, which is alone in bin 0; kNN squared distances reach the clamped bins for clouds far from unit scale.)
+__device__ __forceinline__ int digit(unsigned long long key, int level, int b0) {
+    const int top = b0 == 0 ? 62 : (b0 == kBins - 1 ? 64 : 48);
+    return (int)((key >> (top - 11 * level)) & 0x7FF);
 }
 
 template <int CAP>
@@ -56,7 +66,7 @@ __device__ __forceinline__ int chain_cmp(const SelectSmemT<CAP>& s, unsigned lon
     int b = bin0(key);
     if (b != s.bin_sel[0]) return b < s.bin_sel[0] ? -1 : 1;
     for (int l = 1; l < upto; ++l) {
-        int bl = (int)((key >> (48 - 11 * l)) & 0x7FF);
+        int bl = digit(key, l, b);
         if (bl != s.bin_sel[l]) return bl < s.bin_sel[l] ? -1 : 1;
     }
     return 0;
@@ -73,7 +83,7 @@ __device__ void find_boundary(SelectSmemT<CAP>& s, int N, int k, int cand_cap, K
         for (int i = tid; i < N; i += kThreads) {
             unsigned long long key = keyfn(i);
             if (level == 0) atomicAdd(&s.hist[bin0(key)], 1u);
-            else if (chain_cmp(s, key, level) == 0) atomicAdd(&s.hist[(int)((key >> (48 - 11 * level)) & 0x7FF)], 1u);
+            else if (chain_cmp(s, key, level) == 0) atomicAdd(&s.hist[digit(key, level, s.bin_sel[0])], 1u);
         }
         __syncthreads();
         if (tid < 32) {  // warp 0: locate the bin where the running count crosses k
@@ -331,6 +341,13 @@ __device__ __forceinline__ float u01_open(uint32_t x) {  // (0,1]
     return ((float)(x >> 8) + 1.0f) * (1.0f / 16777216.0f);
 }
 
+// Exp(1) clock from 32 random bits, never negative and never -0: -__logf(u) is -0 at u = 1 and, with __logf's absolute error
+// of 2^-21.4, can be slightly negative just below 1.  Either gives a key with the sign bit set, which sorts last instead of
+// first, so the point would be dropped instead of drawn.
+__device__ __forceinline__ float exp_clock(uint32_t x) {
+    return fmaxf(-__logf(u01_open(x)), 0.0f) + 0.0f;      // + 0 turns a -0 from fmaxf into +0
+}
+
 // ------------------------------------------------------------------------------------------------
 // K2b: ball-query patches (radius ablations) -- point_cloud.get_patch_kdtree with patch_radius > 0
 // (source/base/point_cloud.py:176-192) + the padding rule of PointcloudPatchDataset.__getitem__
@@ -364,7 +381,7 @@ ball_patch_kernel(const float* __restrict__ pts, int N, const float* __restrict_
     auto clock_key = [&](int i) {     // Exp(1) clock of point i for this query
         uint32_t r[4];
         philox4x32_10((uint32_t)seed, (uint32_t)(seed >> 32), (uint32_t)qi, (uint32_t)(qi >> 32), (uint32_t)(i >> 2), 0x3c6ef372u, r);
-        return dkey((double)(-__logf(u01_open(r[i & 3]))));
+        return dkey((double)exp_clock(r[i & 3]));
     };
     if (tid == 0) { s.n_cand = 0; s.n_direct = 0; }
     __syncthreads();
@@ -494,7 +511,7 @@ subsample_weighted_kernel(const float* __restrict__ pts, int N, const float* __r
         return fminf(fmaxf(w, 0.05f), 1.0f);
     };
     // exponential clock with rate w: the S earliest arrivals are a draw without replacement with p ~ w
-    auto clock_of = [&](float w, uint32_t rnd) { return __fdividef(-__logf(u01_open(rnd)), w); };
+    auto clock_of = [&](float w, uint32_t rnd) { return __fdividef(exp_clock(rnd), w); };
     auto philox_block = [&](int i4, uint32_t (&r)[4]) {
         philox4x32_10((uint32_t)seed, (uint32_t)(seed >> 32), (uint32_t)qi, (uint32_t)(qi >> 32), (uint32_t)i4, 0x77f1e2d3u, r);
     };
