@@ -313,7 +313,7 @@ def test_reconstruct_matches_stagewise_oracle(variant):
 
 
 # ------------------------------------------------------------------ a12 : marching cubes (oracle unpinned vs skimage)
-# vertices: fp32 interpolation on both sides, tolerance 1e-6 absolute in model space; faces: identical indices.
+# vertices: the same separately rounded fp32 operations on both sides, so identical bits; faces: identical indices.
 @pytest.mark.parametrize('case', ['sphere', 'noise', 'propagated', 'all_cases'])
 def test_marching_cubes_matches_oracle(case):
     from oracle import mc_oracle as mc
@@ -338,7 +338,7 @@ def test_marching_cubes_matches_oracle(case):
     vo, fo = mc.marching_cubes(vol, 0.0)
     assert v.shape == vo.shape and f.shape == fo.shape
     assert np.array_equal(f.cpu().numpy(), fo)
-    np.testing.assert_allclose(v.cpu().numpy(), vo, rtol=0, atol=1e-6)
+    assert np.array_equal(v.cpu().numpy(), vo)
     assert mc.mesh_is_closed(f.cpu().numpy())
     # the table-free second restatement (oracle/mc_topo.py: polygons traced on the cell values, asymptotic decider on
     # ambiguous faces) shares nothing with tools/gen_mc_tables.py: same vertices, same triangles
