@@ -51,7 +51,9 @@ typedef struct p2s_model p2s_model;
 
 /* Mirrors the constructor arguments of source/points_to_surf_model.py:238-240 as used by
  * source/points_to_surf_eval.py:150-166.  Supported subset (SURVEY.md section 8b): sym_op='max',
- * single_transformer=0, use_feat_stn=1, output_dim=2 (imp_surf_magnitude, imp_surf_sign). */
+ * single_transformer=0, use_feat_stn=1.  The head's output_dim is not part of this struct: the functions without
+ * the _ex suffix mean output_dim=2 (imp_surf_magnitude, imp_surf_sign); the _ex variants also take output_dim=1, the
+ * regression head of the imp_surf ablation (experiments/train_p2s_regression.sh). */
 typedef struct {
     int32_t use_point_stn;      /* train_opt.use_point_stn                                  */
     int32_t shared_transformer; /* train_opt.shared_transformer                             */
@@ -68,21 +70,27 @@ typedef struct {
  *   FEAT(p, qstn) := [STN3(p.stn1) if qstn] STN64(p.stn2) p.conv0a p.conv0b p.conv1 p.conv2 p.conv3
  *   blob := [STN3(point_stn) if use_point_stn && shared_transformer]
  *           FEAT(feat_local, 0)  FEAT(feat_global, use_point_stn && !shared_transformer)
- *           fc1_local fc1_global fc2 fc3 fc4
+ *           fc1_local fc1_global fc2 fc3 fc4            (fc4: 128 -> output_dim)
  * points2surf_b200/weights.py builds it from a reference state_dict. */
 size_t p2s_model_blob_floats(const p2s_model_config* cfg);
+/* the same for a head of output_dim outputs (1 or 2); 0 for any other output_dim */
+size_t p2s_model_blob_floats_ex(const p2s_model_config* cfg, int output_dim);
 
 /* Replaces make_regressor (source/points_to_surf_eval.py:150-171): builds the device-resident,
  * kernel-ready weight set on CUDA device `device`. */
 int p2s_model_create(const p2s_model_config* cfg, const float* blob_host, size_t blob_floats,
                      int device, p2s_model** out);
+/* output_dim 2: p2s_model_create.  output_dim 1: the regression head (outputs imp_surf).  Any other value is an error. */
+int p2s_model_create_ex(const p2s_model_config* cfg, int output_dim, const float* blob_host, size_t blob_floats,
+                        int device, p2s_model** out);
 void p2s_model_destroy(p2s_model* m);
 
 /* Arithmetic of the per-point MLP stacks:
  *   P2S_PRECISION_FP32  CUDA-core fp32 FMA everywhere (accuracy path; also the guard-band recompute path)
  *   P2S_PRECISION_TC    wgmma tensor cores,  fp16 operands (11-bit significand, same as the TF32 the
  *                       reference's cuDNN Conv1d uses on Ampere+), fp32 accumulate; queries whose
- *                       |sign logit| < guard_band are recomputed on the fp32 path. */
+ *                       |sign logit| (output_dim 2) or |logit| (output_dim 1) < guard_band are recomputed on
+ *                       the fp32 path. */
 #define P2S_PRECISION_FP32 0
 #define P2S_PRECISION_TC 1
 int p2s_model_set_precision(p2s_model* m, int precision, float guard_band);
@@ -107,7 +115,8 @@ int p2s_model_set_debug_aux(p2s_model* m, float* aux);
  *   pts_sub_sample_ms       [B, sub_sample_size, 3]    x['pts_sub_sample_ms'] (model space, NOT yet centred;
  *                                                       unlike the reference this op does not modify it)
  *   imp_surf_query_point_ms [B, 3]                     x['imp_surf_query_point_ms']
- *   logits                  [B, 2]                     (|d| logit, sign logit) */
+ *   logits                  [B, output_dim]            (|d| logit, sign logit), or the single signed-distance
+ *                                                       logit of an output_dim 1 model */
 int p2s_forward_dev(p2s_model* m, const float* patch_pts_ps, const float* pts_sub_sample_ms,
                     const float* imp_surf_query_point_ms, int64_t B, float* logits, void* stream);
 int p2s_forward_host(p2s_model* m, const float* patch_pts_ps, const float* pts_sub_sample_ms,
@@ -118,6 +127,11 @@ int p2s_forward_host(p2s_model* m, const float* patch_pts_ps, const float* pts_s
  * (train_opt.patch_radius > 0): the magnitude is not rescaled (points_to_surf_eval.py:188-189,364-368). */
 int p2s_sdf_from_logits_dev(const float* logits, const float* patch_radius_ms, int64_t B,
                             float* sdf, void* stream);
+/* post_process of the regression head (source/sdf_nn.py:6-8, source/points_to_surf_eval.py:176-183,205-207):
+ * logits [B, 1], sdf = tanh(l)^2 * sign(l) * radius with sign(0) = 0, NaN -> 1.  patch_radius_ms == NULL is the
+ * fixed-radius case: not rescaled. */
+int p2s_distance_from_logits_dev(const float* logits, const float* patch_radius_ms, int64_t B,
+                                 float* sdf, void* stream);
 
 /* ------------------------------------------------------------------ query assembly ------------- */
 /* sdf.get_voxel_centers_grid_smaller_pc (source/sdf.py:46-70): candidate voxels within an eps^3 box
@@ -169,7 +183,8 @@ int p2s_gather_points_dev(const float* pts, const int32_t* ids, int64_t count, f
 /* The eval loop of source/points_to_surf_eval.py:337-404 in reconstruction mode for ONE shape:
  * candidate grid -> per query (kNN patch, sub-sample, network, post-process) -> SDF band.
  *   pts [N,3] device;  on return *Q_host queries, lin_idx [cap] and sdf [cap] device arrays filled
- *   (what the reference writes to rec/query_pts_ms and rec/dist_ms).  first_query/num_queries
+ *   (what the reference writes to rec/query_pts_ms and rec/dist_ms).  The post-process follows the model's head:
+ *   p2s_sdf_from_logits_dev for output_dim 2, p2s_distance_from_logits_dev for output_dim 1.  first_query/num_queries
  *   select a contiguous slab of the ordered query list (multi-GPU tile sharding); pass 0,-1 for all.
  * sync: count read-back. */
 typedef struct {

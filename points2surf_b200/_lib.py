@@ -57,6 +57,8 @@ SIGNATURES = {
     'p2s_launch_count_reset': (None, []),
     'p2s_model_blob_floats': (C.c_size_t, [C.POINTER(ModelConfig)]),
     'p2s_model_create': (C.c_int, [C.POINTER(ModelConfig), _vp, C.c_size_t, C.c_int, C.POINTER(_vp)]),
+    'p2s_model_blob_floats_ex': (C.c_size_t, [C.POINTER(ModelConfig), C.c_int]),
+    'p2s_model_create_ex': (C.c_int, [C.POINTER(ModelConfig), C.c_int, _vp, C.c_size_t, C.c_int, C.POINTER(_vp)]),
     'p2s_model_destroy': (None, [_vp]),
     'p2s_model_set_precision': (C.c_int, [_vp, C.c_int, _f32]),
     'p2s_model_last_guard_count': (C.c_int, [_vp, C.POINTER(_i64)]),
@@ -66,6 +68,7 @@ SIGNATURES = {
     'p2s_forward_dev': (C.c_int, [_vp, _vp, _vp, _vp, _i64, _vp, _vp]),
     'p2s_forward_host': (C.c_int, [_vp, _vp, _vp, _vp, _i64, _vp]),
     'p2s_sdf_from_logits_dev': (C.c_int, [_vp, _vp, _i64, _vp, _vp]),
+    'p2s_distance_from_logits_dev': (C.c_int, [_vp, _vp, _i64, _vp, _vp]),
     'p2s_query_grid_dev': (C.c_int, [_vp, _i64, _i32, _i32, _vp, _i64, C.POINTER(_i64), _vp]),
     'p2s_query_points_dev': (C.c_int, [_vp, _i64, _i32, _vp, _vp]),
     'p2s_knn_patch_dev': (C.c_int, [_vp, _i64, _vp, _i64, _i32, _vp, _vp, _vp, _vp]),

@@ -20,6 +20,7 @@ void scatter_f32(const float* src, const int32_t* idx, int64_t n, float* dst, cu
 void gather_points(const float* pts, const int32_t* ids, int64_t count, float* out, cudaStream_t st);
 int assemble_error_check(cudaStream_t st);
 void sdf_from_logits(const float* logits, const float* radius, int64_t B, float* sdf, cudaStream_t st);
+void distance_from_logits(const float* logits, const float* radius, int64_t B, float* sdf, cudaStream_t st);
 void sdf_to_volume(const int32_t* lin_idx, const float* sdf, int64_t Q, int res, int sigma, float thr, float* vol, int* iterations_host, cudaStream_t st);
 void marching_cubes(const float* vol, int res, float level, float* verts, int64_t vcap, int32_t* faces, int64_t fcap, int64_t* nverts_host, int64_t* nfaces_host, cudaStream_t st);
 
@@ -81,13 +82,13 @@ size_t feat_floats(bool qstn, int net) {
     auto l = [](size_t co, size_t ci) { return co * ci + co; };
     return (qstn ? stn_floats(3, 4, net) : 0) + stn_floats(64, 4096, net) + l(64, 3) + l(64, 64) + l(64, 64) + l(128, 64) + l(net, 128);
 }
-size_t blob_floats(const p2s_model_config& c) {
+size_t blob_floats(const p2s_model_config& c, int output_dim) {
     auto l = [](size_t co, size_t ci) { return co * ci + co; };
     const int net = c.net_size;
     const bool shared = c.use_point_stn && c.shared_transformer;
     const bool gq = c.use_point_stn && !c.shared_transformer;
     return (shared ? stn_floats(3, 4, net) : 0) + feat_floats(false, net) + feat_floats(gq, net) +
-           2 * l(net / 2, net) + l(net / 4, net) + l(net / 8, net / 4) + l(2, net / 8);
+           2 * l(net / 2, net) + l(net / 4, net) + l(net / 8, net / 4) + l(output_dim, net / 8);
 }
 
 void check_cfg(const p2s_model_config& c) {
@@ -95,6 +96,8 @@ void check_cfg(const p2s_model_config& c) {
     P2S_CHECK(c.points_per_patch >= 8 && c.points_per_patch <= 1536, "points_per_patch must be in [8, 1536]");
     P2S_CHECK(c.sub_sample_size >= 8 && c.sub_sample_size <= 4096, "sub_sample_size must be in [8, 4096]");
 }
+
+bool output_dim_ok(int output_dim) { return output_dim == 1 || output_dim == 2; }
 
 cudaStream_t as_stream(void* s) { return reinterpret_cast<cudaStream_t>(s); }
 
@@ -110,6 +113,12 @@ void forward(Model& m, const float* patch, const float* sub, const float* query,
     if (B <= 0) return;
     if (m.precision == P2S_PRECISION_TC) forward_tc(m, patch, sub, query, B, logits, st);
     else forward_fp32(m, patch, sub, query, B, logits, st);
+}
+
+// the post-process of the model's head: (|d| logit, sign logit) or the regression head's single logit
+static void logits_to_sdf(const Model& m, const float* logits, const float* radius, int64_t B, float* sdf, cudaStream_t st) {
+    if (m.fc4.cout == 1) distance_from_logits(logits, radius, B, sdf, st);
+    else sdf_from_logits(logits, radius, B, sdf, st);
 }
 
 static void reconstruct(Model& m, const p2s_recon_config& rc, const float* pts, int64_t N, int64_t first_query,
@@ -131,12 +140,13 @@ static void reconstruct(Model& m, const p2s_recon_config& rc, const float* pts, 
     P2S_CUDA(cudaMemcpyAsync(lin_idx, all_idx + first_query, (size_t)Q * 4, cudaMemcpyDeviceToDevice, st));
     int64_t batch = rc.batch > 0 ? rc.batch : (m.precision == P2S_PRECISION_TC ? 8192 : 2048);
     if (batch > Q) batch = Q;
-    size_t per_q = 3 + (size_t)P * 3 + 1 + (size_t)S * 3 + 2 + (size_t)S;
+    const int od = m.fc4.cout;
+    size_t per_q = 3 + (size_t)P * 3 + 1 + (size_t)S * 3 + od + (size_t)S;
     float* base = m.ws_io.as<float>(per_q * (size_t)batch + 64);
     BatchBufs b;
     float* p = base;
     auto take = [&](size_t n) { float* r = p; p += (n * (size_t)batch + 3) / 4 * 4; return r; };
-    b.qpts = take(3); b.patch = take((size_t)P * 3); b.radius = take(1); b.sub = take((size_t)S * 3); b.logits = take(2);
+    b.qpts = take(3); b.patch = take((size_t)P * 3); b.radius = take(1); b.sub = take((size_t)S * 3); b.logits = take(od);
     b.sub_ids = reinterpret_cast<int32_t*>(take((size_t)S));
     // guard band of the tensor-core path: flagged queries are collected over the whole slab and recomputed on the
     // fp32 path in one batch at the end (large GEMMs instead of ~80-query slivers per batch)
@@ -166,7 +176,7 @@ static void reconstruct(Model& m, const p2s_recon_config& rc, const float* pts, 
             assemble(lin_idx + q0, n, first_query + q0, nullptr);
             m.guard_base = q0;
             forward(m, b.patch, b.sub, b.qpts, n, b.logits, st);
-            sdf_from_logits(b.logits, fixed_radius ? nullptr : b.radius, n, sdf + q0, st);
+            logits_to_sdf(m, b.logits, fixed_radius ? nullptr : b.radius, n, sdf + q0, st);
         }
         if (defer_guard) {
             m.guard_list = nullptr;
@@ -183,7 +193,7 @@ static void reconstruct(Model& m, const p2s_recon_config& rc, const float* pts, 
                 gather_i32(lin_idx, glist + g0, n, glin, st);
                 assemble(glin, n, first_query, glist + g0);
                 forward_guard(m, b.patch, b.sub, b.qpts, n, b.logits, st);
-                sdf_from_logits(b.logits, fixed_radius ? nullptr : b.radius, n, gsdf, st);
+                logits_to_sdf(m, b.logits, fixed_radius ? nullptr : b.radius, n, gsdf, st);
                 scatter_f32(gsdf, glist + g0, n, sdf, st);
             }
         }
@@ -207,15 +217,25 @@ uint64_t p2s_launch_count(void) { return g_launches.load(); }
 void p2s_launch_count_reset(void) { g_launches.store(0); }
 
 size_t p2s_model_blob_floats(const p2s_model_config* cfg) {
-    if (!cfg) return 0;
-    return blob_floats(*cfg);
+    return p2s_model_blob_floats_ex(cfg, 2);
+}
+
+size_t p2s_model_blob_floats_ex(const p2s_model_config* cfg, int output_dim) {
+    if (!cfg || !output_dim_ok(output_dim)) return 0;
+    return blob_floats(*cfg, output_dim);
 }
 
 int p2s_model_create(const p2s_model_config* cfg, const float* blob_host, size_t n_floats, int device, p2s_model** out) {
+    return p2s_model_create_ex(cfg, 2, blob_host, n_floats, device, out);
+}
+
+int p2s_model_create_ex(const p2s_model_config* cfg, int output_dim, const float* blob_host, size_t n_floats, int device,
+                        p2s_model** out) {
     return guarded([&] {
         P2S_CHECK(cfg && blob_host && out, "null argument");
         check_cfg(*cfg);
-        P2S_CHECK(n_floats == blob_floats(*cfg), "weight blob size does not match the model config");
+        P2S_CHECK(output_dim_ok(output_dim), "output_dim must be 1 (imp_surf) or 2 (imp_surf_magnitude, imp_surf_sign)");
+        P2S_CHECK(n_floats == blob_floats(*cfg, output_dim), "weight blob size does not match the model config");
         int ndev = 0;
         cudaError_t e = cudaGetDeviceCount(&ndev);
         if (e != cudaSuccess || ndev == 0) throw Error("no CUDA device available: libp2s_b200 has no CPU fallback");
@@ -243,7 +263,7 @@ int p2s_model_create(const p2s_model_config* cfg, const float* blob_host, size_t
         m->fc1_global = c.take(net / 2, net);
         m->fc2 = c.take(net / 4, net);
         m->fc3 = c.take(net / 8, net / 4);
-        m->fc4 = c.take(2, net / 8);
+        m->fc4 = c.take(output_dim, net / 8);
         P2S_CHECK(c.left == 0, "weight blob has trailing data");
         tc_build(*m);
         *out = reinterpret_cast<p2s_model*>(m);
@@ -324,9 +344,9 @@ int p2s_forward_host(p2s_model* mm, const float* patch, const float* sub, const 
         Model* m = reinterpret_cast<Model*>(mm);
         P2S_CUDA(cudaSetDevice(m->device));
         if (B <= 0) return;
-        const size_t P = m->cfg.points_per_patch, S = m->cfg.sub_sample_size;
+        const size_t P = m->cfg.points_per_patch, S = m->cfg.sub_sample_size, od = m->fc4.cout;
         cudaStream_t st = m->own_stream;
-        float* d = m->ws_host.as<float>((size_t)B * (P * 3 + S * 3 + 3 + 2) + 16);
+        float* d = m->ws_host.as<float>((size_t)B * (P * 3 + S * 3 + 3 + od) + 16);
         float* d_patch = d;
         float* d_sub = d_patch + (size_t)B * P * 3;
         float* d_q = d_sub + (size_t)B * S * 3;
@@ -335,7 +355,7 @@ int p2s_forward_host(p2s_model* mm, const float* patch, const float* sub, const 
         P2S_CUDA(cudaMemcpyAsync(d_sub, sub, (size_t)B * S * 3 * 4, cudaMemcpyHostToDevice, st));
         P2S_CUDA(cudaMemcpyAsync(d_q, query, (size_t)B * 3 * 4, cudaMemcpyHostToDevice, st));
         forward(*m, d_patch, d_sub, d_q, B, d_out, st);
-        P2S_CUDA(cudaMemcpyAsync(logits, d_out, (size_t)B * 2 * 4, cudaMemcpyDeviceToHost, st));
+        P2S_CUDA(cudaMemcpyAsync(logits, d_out, (size_t)B * od * 4, cudaMemcpyDeviceToHost, st));
         P2S_CUDA(cudaStreamSynchronize(st));
     });
 }
@@ -344,6 +364,13 @@ int p2s_sdf_from_logits_dev(const float* logits, const float* radius, int64_t B,
     return guarded([&] {
         P2S_CHECK(logits && sdf, "null argument");
         sdf_from_logits(logits, radius, B, sdf, as_stream(stream));
+    });
+}
+
+int p2s_distance_from_logits_dev(const float* logits, const float* radius, int64_t B, float* sdf, void* stream) {
+    return guarded([&] {
+        P2S_CHECK(logits && sdf, "null argument");
+        distance_from_logits(logits, radius, B, sdf, as_stream(stream));
     });
 }
 

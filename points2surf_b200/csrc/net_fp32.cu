@@ -464,7 +464,7 @@ void forward_fp32(Model& m, const float* patch, const float* sub, const float* q
         launch_gemm_nt(w.fb_global, 0, 1024, m.fc1_global.W, 0, m.fc1_global.b, w.cat + 512, 0, 1024, (int)Bc, 512, 1024, 1, true, st);
         fc(m.fc2, w.cat, w.h3, Bc, true, st);
         fc(m.fc3, w.h3, w.h4, Bc, true, st);
-        fc(m.fc4, w.h4, logits + b0 * 2, Bc, false, st);
+        fc(m.fc4, w.h4, logits + b0 * m.fc4.cout, Bc, false, st);   // logits [B][output_dim]
     }
 }
 

@@ -421,10 +421,11 @@ __global__ void transpose64_kernel(const float* __restrict__ in, float* __restri
     out[e] = in[b * 4096 + j * 64 + i];
 }
 
-__global__ void guard_flag_kernel(const float* __restrict__ logits, int64_t B, float band, int32_t* __restrict__ list, int* __restrict__ count, int64_t base, int64_t cap) {
+// logits [B][od]; the sign-deciding logit is the last column (od 2: the sign logit, od 1: the signed-distance logit)
+__global__ void guard_flag_kernel(const float* __restrict__ logits, int od, int64_t B, float band, int32_t* __restrict__ list, int* __restrict__ count, int64_t base, int64_t cap) {
     int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= B) return;
-    if (fabsf(logits[i * 2 + 1]) < band) {
+    if (fabsf(logits[i * od + od - 1]) < band) {
         int slot = atomicAdd(count, 1);
         if (slot < cap) list[slot] = (int32_t)(base + i);
     }
@@ -435,11 +436,10 @@ __global__ void guard_gather_kernel(const float* __restrict__ src, const int32_t
     int i = (int)(e / row_floats), j = (int)(e % row_floats);
     dst[e] = src[(int64_t)list[i] * row_floats + j];
 }
-__global__ void guard_scatter_kernel(const float* __restrict__ src, const int32_t* __restrict__ list, int n, float* __restrict__ logits) {
+__global__ void guard_scatter_kernel(const float* __restrict__ src, const int32_t* __restrict__ list, int n, int od, float* __restrict__ logits) {
     int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
-    logits[(int64_t)list[i] * 2 + 0] = src[i * 2 + 0];
-    logits[(int64_t)list[i] * 2 + 1] = src[i * 2 + 1];
+    for (int j = 0; j < od; ++j) logits[(int64_t)list[i] * od + j] = src[i * od + j];
 }
 __global__ void guard_scatter_rows_kernel(const float* __restrict__ src, const int32_t* __restrict__ list, int n, int row_floats, float* __restrict__ dst) {
     int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -798,7 +798,8 @@ static void forward_tc_core(Model& m, const float* patch, const float* sub, cons
             run_fc(t.head_fc2, cat, 1024, h3, 256, Bc, true, fc_tc, st);
             run_fc(t.head_fc3, h3, 256, h4, 128, Bc, true, fc_tc, st);
         }
-        launch_gemm_nt(h4, 0, 128, m.fc4.W, 0, m.fc4.b, logits + b0 * 2, 0, 2, (int)Bc, 2, 128, 1, false, st);
+        const int od = m.fc4.cout;
+        launch_gemm_nt(h4, 0, 128, m.fc4.W, 0, m.fc4.b, logits + b0 * od, 0, od, (int)Bc, od, 128, 1, false, st);
     }
 }
 
@@ -812,19 +813,19 @@ void forward_guard(Model& m, const float* patch, const float* sub, const float* 
 
 void forward_tc(Model& m, const float* patch, const float* sub, const float* query, int64_t B,
                 float* logits, cudaStream_t st) {
-    const int P = m.cfg.points_per_patch, S = m.cfg.sub_sample_size;
+    const int P = m.cfg.points_per_patch, S = m.cfg.sub_sample_size, od = m.fc4.cout;
     forward_tc_core(m, patch, sub, query, B, logits, st, false);
 
-    // guard band: queries whose sign logit is too close to 0 for fp16-operand arithmetic are recomputed in fp32
+    // guard band: queries whose sign-deciding logit is too close to 0 for fp16-operand arithmetic are recomputed in fp32
     if (m.guard_band > 0.f && m.guard_list) {
         // deferred: only record which queries fall into the band (the fused pipeline recomputes them in one batch)
-        P2S_LAUNCH(guard_flag_kernel, (unsigned)cdiv(B, 256), 256, 0, st, logits, B, m.guard_band, m.guard_list, m.guard_list_count, m.guard_base, m.guard_list_cap);
+        P2S_LAUNCH(guard_flag_kernel, (unsigned)cdiv(B, 256), 256, 0, st, logits, od, B, m.guard_band, m.guard_list, m.guard_list_count, m.guard_base, m.guard_list_cap);
     } else if (m.guard_band > 0.f) {
         StageScope ts_guard("net: guard-band fp32 recompute", st);
         int32_t* list = m.ws_guard.as<int32_t>((size_t)B + 64);
         int* count = reinterpret_cast<int*>(list + B);
         P2S_CUDA(cudaMemsetAsync(count, 0, sizeof(int), st));
-        P2S_LAUNCH(guard_flag_kernel, (unsigned)cdiv(B, 256), 256, 0, st, logits, B, m.guard_band, list, count, (int64_t)0, B);
+        P2S_LAUNCH(guard_flag_kernel, (unsigned)cdiv(B, 256), 256, 0, st, logits, od, B, m.guard_band, list, count, (int64_t)0, B);
         int n = 0;
         P2S_CUDA(cudaMemcpyAsync(&n, count, sizeof(int), cudaMemcpyDeviceToHost, st));
         P2S_CUDA(cudaStreamSynchronize(st));
@@ -833,9 +834,9 @@ void forward_tc(Model& m, const float* patch, const float* sub, const float* que
             const size_t rowp = (size_t)P * 3, rows = (size_t)S * 3;
             float* const aux = m.debug_aux;
             const size_t aux_floats = aux ? (size_t)n * kAuxStride : 0;
-            float* gbuf = m.ws_misc.as<float>((size_t)n * (rowp + rows + 3 + 2) + 64 + aux_floats);
+            float* gbuf = m.ws_misc.as<float>((size_t)n * (rowp + rows + 3 + od) + 64 + aux_floats);
             float* gp = gbuf; float* gs = gp + (size_t)n * rowp; float* gq = gs + (size_t)n * rows; float* gl = gq + ((size_t)n * 3 + 3) / 4 * 4;
-            float* gaux = gl + ((size_t)n * 2 + 3) / 4 * 4;
+            float* gaux = gl + ((size_t)n * od + 3) / 4 * 4;
             P2S_LAUNCH(guard_gather_kernel, (unsigned)cdiv((int64_t)n * rowp, 256), 256, 0, st, patch, list, n, (int)rowp, gp);
             P2S_LAUNCH(guard_gather_kernel, (unsigned)cdiv((int64_t)n * rows, 256), 256, 0, st, sub, list, n, (int)rows, gs);
             P2S_LAUNCH(guard_gather_kernel, (unsigned)cdiv((int64_t)n * 3, 256), 256, 0, st, query, list, n, 3, gq);
@@ -849,7 +850,7 @@ void forward_tc(Model& m, const float* patch, const float* sub, const float* que
                 throw;
             }
             m.debug_aux = aux;
-            P2S_LAUNCH(guard_scatter_kernel, (unsigned)cdiv(n, 256), 256, 0, st, gl, list, n, logits);
+            P2S_LAUNCH(guard_scatter_kernel, (unsigned)cdiv(n, 256), 256, 0, st, gl, list, n, od, logits);
             if (aux) P2S_LAUNCH(guard_scatter_rows_kernel, (unsigned)cdiv((int64_t)n * kAuxStride, 256), 256, 0, st, gaux, list, n, (int)kAuxStride, aux);
         }
     }

@@ -1,5 +1,6 @@
 // K6 / K7: SDF epilogue, scatter into the dense volume, iterative sign propagation.
 //   post_process + combine       source/sdf_nn.py:11-21, source/points_to_surf_eval.py:184-196,263-271,205-207
+//   post_process (regression)    source/sdf_nn.py:6-8, source/points_to_surf_eval.py:176-183,205-207
 //   add_samples_to_volume        source/sdf.py:82-111 (reconstruction case: one sample per voxel -> scatter)
 //   propagate_sign               source/sdf.py:114-178
 //   clamp                        source/sdf.py:200-202
@@ -24,6 +25,20 @@ __global__ void sdf_from_logits_kernel(const float* __restrict__ logits, const f
     if (radius) mag = __fmul_rn(mag, radius[i]);
     float v = logits[i * 2 + 1] >= 0.0f ? mag : -mag;
     if (isnan(v)) v = 1.0f;  // points_to_surf_eval.py:205-207
+    sdf[i] = v;
+}
+
+// regression head (outputs imp_surf): sdf = tanh(l)^2 * sign(l) * radius with sign(0) = 0, in the reference's order of
+// operations (sdf_nn.py:6-8, points_to_surf_eval.py:176-183); NaN -> 1 (points_to_surf_eval.py:205-207)
+__global__ void distance_from_logits_kernel(const float* __restrict__ logits, const float* __restrict__ radius,
+                                            int64_t B, float* __restrict__ sdf) {
+    int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= B) return;
+    const float l = logits[i];
+    const float t = tanhf(l);
+    float v = __fmul_rn(__fmul_rn(t, t), l > 0.0f ? 1.0f : (l < 0.0f ? -1.0f : 0.0f));
+    if (radius) v = __fmul_rn(v, radius[i]);
+    if (isnan(v)) v = 1.0f;
     sdf[i] = v;
 }
 
@@ -584,6 +599,11 @@ __global__ void finalize_kernel(float* __restrict__ vol, const uint8_t* __restri
 void sdf_from_logits(const float* logits, const float* radius, int64_t B, float* sdf, cudaStream_t st) {
     if (B <= 0) return;
     P2S_LAUNCH(sdf_from_logits_kernel, (unsigned)cdiv(B, 256), 256, 0, st, logits, radius, B, sdf);
+}
+
+void distance_from_logits(const float* logits, const float* radius, int64_t B, float* sdf, cudaStream_t st) {
+    if (B <= 0) return;
+    P2S_LAUNCH(distance_from_logits_kernel, (unsigned)cdiv(B, 256), 256, 0, st, logits, radius, B, sdf);
 }
 
 void sdf_to_volume(const int32_t* lin_idx, const float* sdf, int64_t Q, int res, int sigma, float thr,

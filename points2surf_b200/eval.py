@@ -67,10 +67,22 @@ def _load_train_opt(param_filename):
     return train_opt
 
 
+def _output_dim(train_opt):
+    """Network outputs of a supported checkpoint: 1 for the regression head (imp_surf), 2 for magnitude + sign."""
+    return 1 if 'imp_surf' in train_opt.outputs else 2
+
+
 def _check_supported(train_opt, eval_opt):
     outs = list(train_opt.outputs)
-    if 'imp_surf' in outs or 'imp_surf_magnitude' not in outs or 'imp_surf_sign' not in outs:
-        raise ValueError('Unsupported outputs %s: need imp_surf_magnitude + imp_surf_sign' % outs)
+    if 'imp_surf' in outs:
+        # the regression ablation (experiments/eval_p2s_regression.sh); save_evaluation indexes the patch_pts_ids and
+        # p_index outputs (points_to_surf_eval.py:287-288), so the reference needs them too
+        if 'imp_surf_magnitude' in outs or 'imp_surf_sign' in outs or outs.count('imp_surf') > 1:
+            raise ValueError('Unsupported outputs %s: imp_surf together with imp_surf_magnitude / imp_surf_sign' % outs)
+        if 'patch_pts_ids' not in outs or 'p_index' not in outs:
+            raise ValueError('Unsupported outputs %s: imp_surf needs patch_pts_ids and p_index' % outs)
+    elif 'imp_surf_magnitude' not in outs or 'imp_surf_sign' not in outs:
+        raise ValueError('Unsupported outputs %s: need imp_surf_magnitude + imp_surf_sign, or imp_surf' % outs)
     if getattr(train_opt, 'sym_op', 'max') != 'max':
         raise ValueError('Unsupported symmetric operation: %s' % train_opt.sym_op)
     if getattr(train_opt, 'single_transformer', 0):
@@ -149,7 +161,7 @@ def _reconstruct_fixed_subsample(eng, train_opt, eval_opt, pts_dev):
         q = q_all[b0:b0 + bs].contiguous()
         patch, radius = _patches(pts_dev, q, train_opt, eval_opt.seed, query_index_base=b0)
         sub = _fixed_sub(pts_dev, q.shape[0], train_opt.sub_sample_size)
-        out.append(ops.sdf_from_logits(eng.forward(patch, sub, q), radius))
+        out.append(eng.post_process(eng.forward(patch, sub, q), radius))
     sdf = torch.cat(out) if out else torch.zeros((0,), dtype=torch.float32, device=pts_dev.device)
     return lin, sdf
 
@@ -170,7 +182,7 @@ def _eval_given_queries(eng, train_opt, eval_opt, pts_dev, query_pts, dev):
     bs = eval_opt.batchSize if eval_opt.batchSize > 0 else 4096
     for b0 in range(0, q.shape[0], bs):
         out.append(eng.forward(patch[b0:b0 + bs], sub[b0:b0 + bs], qr[b0:b0 + bs]))
-    return ops.sdf_from_logits(torch.cat(out), radius)
+    return eng.post_process(torch.cat(out), radius)
 
 
 def points_to_surf_eval(eval_opt):
@@ -198,7 +210,8 @@ def points_to_surf_eval(eval_opt):
         eng = ops.Engine(state, train_opt.use_point_stn, train_opt.shared_transformer,
                          points_per_patch=train_opt.points_per_patch, sub_sample_size=train_opt.sub_sample_size,
                          net_size=getattr(train_opt, 'net_size', 1024), device=dev_index,
-                         precision=getattr(eval_opt, 'precision', 'tc'), guard_band=getattr(eval_opt, 'guard_band', 0.05))
+                         precision=getattr(eval_opt, 'precision', 'tc'), guard_band=getattr(eval_opt, 'guard_band', 0.05),
+                         output_dim=_output_dim(train_opt))
         uniform = bool(getattr(train_opt, 'uniform_subsample', 0))
         model_out_dir = os.path.join(eval_opt.outdir, 'rec' if eval_opt.reconstruction else 'eval')
         os.makedirs(model_out_dir, exist_ok=True)
@@ -241,6 +254,8 @@ def points_to_surf_eval(eval_opt):
                     query_pts = np.ascontiguousarray(query_pts[inds])
                     np.savetxt(os.path.join(model_out_dir, name + '.idx'), inds, fmt='%d')   # points_to_surf_eval.py:292-294
                 sdf = _eval_given_queries(eng, train_opt, eval_opt, pts_dev, query_pts, dev)
+            # the same files for both heads (save_evaluation's imp and magnitude/sign branches, points_to_surf_eval.py:238-290);
+            # the post-process kernels already map NaN to 1, so the branches' different NaN handling of eval/ cannot show
             imp_surf_np_ms = sdf.cpu().numpy()
             os.makedirs(os.path.join(model_out_dir, 'eval'), exist_ok=True)
             np.save(os.path.join(model_out_dir, 'eval', name + '.xyz.npy'), imp_surf_np_ms)

@@ -3,7 +3,8 @@ signature (points_to_surf_model.py:238-240), parameter names and shapes (so the 
 with or without the DataParallel 'module.' prefix), whose forward runs on the CUDA kernels.
 
 Supported subset (SURVEY.md section 8b): sym_op='max', single_transformer=False, use_feat_stn=True,
-output_dim=2.  Anything else raises ValueError like the reference does for unknown options
+output_dim 2 (imp_surf_magnitude, imp_surf_sign) or 1 (imp_surf, the regression ablation; forward returns [B, 1]
+logits, evaluated with ops.distance_from_logits).  Anything else raises ValueError like the reference does for unknown options
 (points_to_surf_model.py:175).  Inference only: forward() ignores .train() and always uses running
 BatchNorm statistics (the reference evaluates with .eval(), points_to_surf_eval.py:170).
 """
@@ -29,8 +30,9 @@ class PointsToSurfModel(nn.Module):
             raise ValueError('Unsupported option: single_transformer=1 (shared encoder ablation)')
         if not use_feat_stn:
             raise ValueError('Unsupported option: use_feat_stn=0')
-        if output_dim != 2:
-            raise ValueError('Unsupported output_dim %d: only (imp_surf_magnitude, imp_surf_sign) is supported' % output_dim)
+        if output_dim not in (1, 2):
+            raise ValueError('Unsupported output_dim %d: only (imp_surf_magnitude, imp_surf_sign) or imp_surf is supported'
+                             % output_dim)
         if net_size_max != 1024:
             raise ValueError('Unsupported net_size %d' % net_size_max)
         self.net_size_max = net_size_max
@@ -42,6 +44,7 @@ class PointsToSurfModel(nn.Module):
         self.single_transformer = False
         self.shared_transformation = bool(shared_transformation)
         self.precision, self.guard_band = precision, guard_band
+        self.output_dim = output_dim
         for name, kind, cout, cin in arch.layer_specs(self.use_point_stn, self.shared_transformation, net_size_max, output_dim):
             parent = self
             parts = name.split('.')
@@ -77,7 +80,7 @@ class PointsToSurfModel(nn.Module):
             self._engine = ops.Engine(self.state_dict(), self.use_point_stn, self.shared_transformation,
                                       points_per_patch=self.num_points, sub_sample_size=self.sub_sample_size,
                                       net_size=self.net_size_max, device=device.index or 0,
-                                      precision=self.precision, guard_band=self.guard_band)
+                                      precision=self.precision, guard_band=self.guard_band, output_dim=self.output_dim)
             self._engine_key = key
         return self._engine
 

@@ -30,20 +30,23 @@ class Engine:
     """Device-resident model (replaces make_regressor, source/points_to_surf_eval.py:150-171)."""
 
     def __init__(self, state_dict, use_point_stn, shared_transformer, points_per_patch=300,
-                 sub_sample_size=1000, net_size=1024, device=0, precision='fp32', guard_band=0.0):
+                 sub_sample_size=1000, net_size=1024, device=0, precision='fp32', guard_band=0.0, output_dim=2):
+        """output_dim 2: logits (|d| logit, sign logit); output_dim 1: the regression head's signed-distance logit.
+        reconstruct() applies the matching post-process."""
         self.lib = _lib.load()
         if not torch.cuda.is_available():
             raise P2SError('CUDA is not available: points2surf_b200 has no CPU fallback')
         self.device = torch.device('cuda', device if isinstance(device, int) else torch.device(device).index or 0)
         self.cfg = ModelConfig(int(bool(use_point_stn)), int(bool(shared_transformer)), int(points_per_patch),
                                int(sub_sample_size), int(net_size))
-        blob = _weights.pack_blob(state_dict, use_point_stn, shared_transformer)
-        expect = self.lib.p2s_model_blob_floats(C.byref(self.cfg))
+        self.output_dim = int(output_dim)
+        blob = _weights.pack_blob(state_dict, use_point_stn, shared_transformer, self.output_dim)
+        expect = self.lib.p2s_model_blob_floats_ex(C.byref(self.cfg), self.output_dim)
         if blob.size != expect:
             raise P2SError('state_dict does not match the model config (%d floats, expected %d)' % (blob.size, expect))
         h = C.c_void_p()
-        check(self.lib.p2s_model_create(C.byref(self.cfg), blob.ctypes.data_as(C.c_void_p), blob.size,
-                                        self.device.index, C.byref(h)))
+        check(self.lib.p2s_model_create_ex(C.byref(self.cfg), self.output_dim, blob.ctypes.data_as(C.c_void_p), blob.size,
+                                           self.device.index, C.byref(h)))
         self.handle = h
         self.P, self.S = int(points_per_patch), int(sub_sample_size)
         self.set_precision(precision, guard_band)
@@ -97,7 +100,7 @@ class Engine:
         B = pa.shape[0]
         if pa.shape != (B, self.P, 3) or su.shape != (B, self.S, 3) or qu.shape != (B, 3):
             raise P2SError('bad input shapes %s %s %s' % (tuple(pa.shape), tuple(su.shape), tuple(qu.shape)))
-        out = torch.empty((B, 2), dtype=torch.float32, device=pa.device)
+        out = torch.empty((B, self.output_dim), dtype=torch.float32, device=pa.device)
         if B == 0:
             return out
         with torch.cuda.device(pa.device):
@@ -109,10 +112,14 @@ class Engine:
         su = np.ascontiguousarray(pts_sub_sample_ms, dtype=np.float32)
         qu = np.ascontiguousarray(imp_surf_query_point_ms, dtype=np.float32)
         B = pa.shape[0]
-        out = np.empty((B, 2), dtype=np.float32)
+        out = np.empty((B, self.output_dim), dtype=np.float32)
         vp = lambda a: a.ctypes.data_as(C.c_void_p)
         check(self.lib.p2s_forward_host(self.handle, vp(pa), vp(su), vp(qu), B, vp(out)))
         return out
+
+    def post_process(self, logits, patch_radius):
+        """The post-process of this model's head: sdf_from_logits (output_dim 2) or distance_from_logits (output_dim 1)."""
+        return (distance_from_logits if self.output_dim == 1 else sdf_from_logits)(logits, patch_radius)
 
     # ---- fused a1..a9 ----
     def reconstruct(self, pts, res, eps, uniform_subsample, seed, first_query=0, num_queries=-1, batch=0, cap=None,
@@ -161,6 +168,22 @@ def sdf_from_logits(logits, patch_radius):
     out = torch.empty((lg.shape[0],), dtype=torch.float32, device=lg.device)
     with torch.cuda.device(lg.device):
         check(_lib.load().p2s_sdf_from_logits_dev(_ptr(lg), _ptr(r) if r is not None else None, lg.shape[0], _ptr(out), _stream()))
+    return out
+
+
+def distance_from_logits(logits, patch_radius):
+    """Regression head (outputs imp_surf): logits [B,1] -> tanh(l)^2 * sign(l) * radius, NaN -> 1
+    (source/sdf_nn.py:6-8, points_to_surf_eval.py:176-183,205-207).  patch_radius None = fixed-radius patches: not rescaled."""
+    lg = _dev(logits, torch.float32, 'logits')
+    if lg.dim() != 2 or lg.shape[1] != 1:
+        raise P2SError('logits must have shape [B, 1], got %s' % (tuple(lg.shape),))
+    r = _dev(patch_radius, torch.float32, 'patch_radius') if patch_radius is not None else None
+    if r is not None and r.shape != (lg.shape[0],):
+        raise P2SError('patch_radius must have shape [B]')
+    out = torch.empty((lg.shape[0],), dtype=torch.float32, device=lg.device)
+    with torch.cuda.device(lg.device):
+        check(_lib.load().p2s_distance_from_logits_dev(_ptr(lg), _ptr(r) if r is not None else None, lg.shape[0], _ptr(out),
+                                                        _stream()))
     return out
 
 

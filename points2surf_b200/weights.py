@@ -48,8 +48,14 @@ def _feat(sd, p, qstn):
     return out
 
 
-def pack_blob(state_dict, use_point_stn, shared_transformer):
+def pack_blob(state_dict, use_point_stn, shared_transformer, output_dim=2):
+    """output_dim: 2 for the (imp_surf_magnitude, imp_surf_sign) head, 1 for the regression head (imp_surf)."""
     sd = strip_module_prefix(state_dict)
+    if output_dim not in (1, 2):
+        raise ValueError('Unsupported output_dim %r: 1 (imp_surf) or 2 (imp_surf_magnitude, imp_surf_sign)' % (output_dim,))
+    fc4 = tuple(_np(sd['fc4.weight']).shape)
+    if fc4[0] != output_dim:
+        raise ValueError('fc4 has %d outputs, expected output_dim %d' % (fc4[0], output_dim))
     parts = []
     if use_point_stn and shared_transformer:
         parts += _stn(sd, 'point_stn.')
