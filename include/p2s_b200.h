@@ -441,6 +441,11 @@ int p2s_op_maxpool_bwd(const float* dout, const int32_t* arg, int64_t B, int npt
 int p2s_op_loss(const float* pred, const float* target_mag, const float* radius, const float* target_sign,
                 int64_t B, float w_mag, float w_sign, int fixed_radius, double* loss_out, float* dpred,
                 void* stream);
+/* compute_loss for the regression output imp_surf, source/points_to_surf_train.py:541-548 and sdf_nn.calc_loss_distance:
+ * loss_out (device f64 [1]) = w * mse(tanh p, tanh(t/r)) with the signed tanh; dpred [B,1] = its gradient (NULL: forward
+ * only).  fixed_radius != 0 skips the division by r (radius may then be NULL). */
+int p2s_op_loss_distance(const float* pred, const float* target, const float* radius, int64_t B, float w,
+                         int fixed_radius, double* loss_out, float* dpred, void* stream);
 /* utils.batch_quat_to_rotmat (source/base/utils.py:13-46) forward and backward.  q4 [B,4] is the raw fc3 output of the
  * QSTN; the identity quaternion (1,0,0,0) is added inside (source/points_to_surf_model.py:124-126).  R, dR [B,9]. */
 int p2s_op_quat_to_rot(const float* q4, float* R, int64_t B, void* stream);

@@ -95,6 +95,7 @@ SIGNATURES = {
     'p2s_op_maxpool_fwd': (C.c_int, [_vp, _i64, _i32, _i32, _vp, _vp, _vp]),
     'p2s_op_maxpool_bwd': (C.c_int, [_vp, _vp, _i64, _i32, _i32, _vp, _vp]),
     'p2s_op_loss': (C.c_int, [_vp, _vp, _vp, _vp, _i64, _f32, _f32, _i32, _vp, _vp, _vp]),
+    'p2s_op_loss_distance': (C.c_int, [_vp, _vp, _vp, _i64, _f32, _i32, _vp, _vp, _vp]),
     'p2s_op_quat_to_rot': (C.c_int, [_vp, _vp, _i64, _vp]),
     'p2s_op_quat_to_rot_bwd': (C.c_int, [_vp, _vp, _i64, _vp, _vp]),
     'p2s_op_add_row': (C.c_int, [_vp, _vp, _i64, _i32, _vp]),

@@ -2,6 +2,23 @@
 module structure of source/points_to_surf_model.py:12-36,72-99,134-167,237-294."""
 
 
+def head_output_dim(outputs):
+    """The supported `--outputs` lists of a checkpoint, shared by training and evaluation so that every checkpoint the
+    training writes can be evaluated: -> 1 for the regression head (imp_surf), 2 for magnitude + sign; else ValueError."""
+    outs = list(outputs)
+    if 'imp_surf' in outs:
+        # the regression ablation (experiments/*_p2s_regression.sh); the reference's save_evaluation indexes the
+        # patch_pts_ids and p_index outputs (points_to_surf_eval.py:287-288), so it needs them too
+        if 'imp_surf_magnitude' in outs or 'imp_surf_sign' in outs or outs.count('imp_surf') > 1:
+            raise ValueError('Unsupported outputs %s: imp_surf together with imp_surf_magnitude / imp_surf_sign' % outs)
+        if 'patch_pts_ids' not in outs or 'p_index' not in outs:
+            raise ValueError('Unsupported outputs %s: imp_surf needs patch_pts_ids and p_index' % outs)
+        return 1
+    if 'imp_surf_magnitude' not in outs or 'imp_surf_sign' not in outs:
+        raise ValueError('Unsupported outputs %s: need imp_surf_magnitude + imp_surf_sign, or imp_surf' % outs)
+    return 2
+
+
 def layer_specs(use_point_stn, shared_transformation, net=1024, output_dim=2):
     """-> list of (dotted name, kind in {'conv','fc','bn'}, cout, cin) in state_dict order."""
 

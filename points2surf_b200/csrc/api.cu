@@ -584,6 +584,10 @@ P2S_OP(p2s_op_loss, (const float* pred, const float* target_mag, const float* ra
                      float w_mag, float w_sign, int fixed_radius, double* loss_out, float* dpred, void* stream),
        P2S_CHECK(pred && target_mag && target_sign && loss_out && (radius || fixed_radius) && B > 0, "bad argument");
         op_loss(pred, target_mag, radius, target_sign, B, w_mag, w_sign, fixed_radius != 0, loss_out, dpred, as_stream(stream)))
+P2S_OP(p2s_op_loss_distance, (const float* pred, const float* target, const float* radius, int64_t B, float w, int fixed_radius,
+                              double* loss_out, float* dpred, void* stream),
+       P2S_CHECK(pred && target && loss_out && (radius || fixed_radius) && B > 0, "bad argument");
+        op_loss_distance(pred, target, radius, B, w, fixed_radius != 0, loss_out, dpred, as_stream(stream)))
 P2S_OP(p2s_op_quat_to_rot, (const float* q4, float* R, int64_t B, void* stream),
        P2S_CHECK(q4 && R, "null argument"); launch_quat_to_rot(q4, R, B, as_stream(stream)))
 P2S_OP(p2s_op_quat_to_rot_bwd, (const float* q4, const float* dR, int64_t B, float* dq, void* stream),

@@ -154,6 +154,8 @@ void op_maxpool_fwd(const float* y, int64_t B, int npts, int C, float* out, int3
 void op_maxpool_bwd(const float* dout, const int32_t* arg, int64_t B, int npts, int C, float* dy, cudaStream_t st);
 void op_loss(const float* pred, const float* target_mag, const float* radius, const float* target_sign, int64_t B,
              float w_mag, float w_sign, bool fixed_radius, double* loss_out, float* dpred, cudaStream_t st);
+void op_loss_distance(const float* pred, const float* target, const float* radius, int64_t B, float w, bool fixed_radius,
+                      double* loss_out, float* dpred, cudaStream_t st);
 void op_quat_to_rot_bwd(const float* q4, const float* dR, int64_t B, float* dq, cudaStream_t st);
 void op_add_row(float* x, const float* v, int64_t B, int C, cudaStream_t st);
 void op_sgd(float* p, const float* g, float* buf, int64_t n, float lr, float momentum, bool first, cudaStream_t st);

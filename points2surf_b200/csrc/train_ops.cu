@@ -340,6 +340,33 @@ loss_kernel(const float* __restrict__ pred, const float* __restrict__ target_mag
     }
 }
 
+// ---------------------------------------------------------------- regression loss (sdf_nn.calc_loss_distance)
+// loss_out[0] = w * mean((tanh p - tanh(t / r))^2) with the signed tanh (no abs); dpred [B,1] = d loss / d pred =
+// w * 2 (tanh p - tanh t')(1 - tanh^2 p) / B.  One block of 256 threads strides over any B: the per-rank batches of the
+// training step are a few hundred to a few thousand queries, far too little work to split over CTAs.
+__global__ void __launch_bounds__(256)
+loss_distance_kernel(const float* __restrict__ pred, const float* __restrict__ target, const float* __restrict__ radius,
+                     int64_t B, float w, int fixed_radius, double* __restrict__ loss_out, float* __restrict__ dpred) {
+    double l = 0.0;
+    const float invB = 1.f / (float)B;
+    for (int64_t i = threadIdx.x; i < B; i += blockDim.x) {
+        float t = target[i];
+        if (!fixed_radius) t = t / radius[i];
+        const float a = tanhf(pred[i]), b = tanhf(t);
+        const float d = a - b;
+        l += (double)(d * d);
+        if (dpred) dpred[i] = w * 2.f * d * invB * (1.f - a * a);
+    }
+    __shared__ double r[256];
+    r[threadIdx.x] = l;
+    __syncthreads();
+    for (int o = 128; o > 0; o >>= 1) {
+        if (threadIdx.x < o) r[threadIdx.x] += r[threadIdx.x + o];
+        __syncthreads();
+    }
+    if (threadIdx.x == 0) loss_out[0] = (double)w * r[0] / (double)B;
+}
+
 // ---------------------------------------------------------------- quaternion -> rotation, backward
 // R = I + s * A(q), s = 2 / |q|^2 (utils.batch_quat_to_rotmat, source/base/utils.py:13-46; q is not normalised);
 // like the forward kernel, q4 is the raw fc3 output and q = q4 + (1,0,0,0) (points_to_surf_model.py:124-126)
@@ -523,6 +550,11 @@ void op_loss(const float* pred, const float* target_mag, const float* radius, co
              float w_mag, float w_sign, bool fixed_radius, double* loss_out, float* dpred, cudaStream_t st) {
     P2S_LAUNCH(loss_kernel, 1, 256, 0, st, pred, target_mag, radius, target_sign, B, w_mag, w_sign,
                fixed_radius ? 1 : 0, loss_out, dpred);
+}
+
+void op_loss_distance(const float* pred, const float* target, const float* radius, int64_t B, float w, bool fixed_radius,
+                      double* loss_out, float* dpred, cudaStream_t st) {
+    P2S_LAUNCH(loss_distance_kernel, 1, 256, 0, st, pred, target, radius, B, w, fixed_radius ? 1 : 0, loss_out, dpred);
 }
 
 void op_quat_to_rot_bwd(const float* q4, const float* dR, int64_t B, float* dq, cudaStream_t st) {

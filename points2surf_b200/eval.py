@@ -17,6 +17,7 @@ import random
 import numpy as np
 import torch
 
+from . import arch
 from . import ops
 from . import samplers
 from . import sdf as p2s_sdf
@@ -73,16 +74,7 @@ def _output_dim(train_opt):
 
 
 def _check_supported(train_opt, eval_opt):
-    outs = list(train_opt.outputs)
-    if 'imp_surf' in outs:
-        # the regression ablation (experiments/eval_p2s_regression.sh); save_evaluation indexes the patch_pts_ids and
-        # p_index outputs (points_to_surf_eval.py:287-288), so the reference needs them too
-        if 'imp_surf_magnitude' in outs or 'imp_surf_sign' in outs or outs.count('imp_surf') > 1:
-            raise ValueError('Unsupported outputs %s: imp_surf together with imp_surf_magnitude / imp_surf_sign' % outs)
-        if 'patch_pts_ids' not in outs or 'p_index' not in outs:
-            raise ValueError('Unsupported outputs %s: imp_surf needs patch_pts_ids and p_index' % outs)
-    elif 'imp_surf_magnitude' not in outs or 'imp_surf_sign' not in outs:
-        raise ValueError('Unsupported outputs %s: need imp_surf_magnitude + imp_surf_sign, or imp_surf' % outs)
+    arch.head_output_dim(train_opt.outputs)
     if getattr(train_opt, 'sym_op', 'max') != 'max':
         raise ValueError('Unsupported symmetric operation: %s' % train_opt.sym_op)
     if getattr(train_opt, 'single_transformer', 0):

@@ -13,7 +13,8 @@ the reference bit for bit (`tests/golden/samplers.npz`, `tests/golden/train_init
 Status: the host logic is exercised on the CPU with the test primitives (tests/test_train_loop.py); the GPU assembly branch
 has not been run on hardware yet (no GPU budget was left when it was written) -- see DESIGN.md section 7.
 
-Supported configuration: the subset of points2surf_b200.train (kNN patches, `max` pooling, magnitude + sign outputs).
+Supported configuration: the subset of points2surf_b200.train (`max` pooling; magnitude + sign outputs, or the regression
+output `imp_surf` with `patch_pts_ids` and `p_index`, the output lists points2surf_b200.eval accepts).
 """
 import argparse
 import math
@@ -95,8 +96,7 @@ def _check_supported(opt):
     for o in outs:
         if o not in ('imp_surf', 'imp_surf_magnitude', 'imp_surf_sign', 'p_index', 'patch_pts_ids'):
             raise ValueError('Unknown output: %s' % o)
-    if 'imp_surf' in outs or 'imp_surf_magnitude' not in outs or 'imp_surf_sign' not in outs:
-        raise ValueError('Unsupported outputs %s: need imp_surf_magnitude + imp_surf_sign (no imp_surf regression)' % outs)
+    arch.head_output_dim(outs)          # the rule of points2surf_b200.eval: every checkpoint written can be evaluated
     if opt.sym_op != 'max':
         raise ValueError('Unsupported symmetric operation: %s' % opt.sym_op)
     if opt.single_transformer:
@@ -194,7 +194,7 @@ def _random_rotations(rng, n):
 def _assemble_batch(dataset, indices, assembler, rng, device, dtype=torch.float32):
     """The batch dict PointcloudPatchDataset.__getitem__ + the default collate produce for these global patch indices
     (source/data_loader.py:352-421): keys patch_pts_ps, patch_radius_ms, pts_sub_sample_ms, imp_surf_query_point_ms,
-    imp_surf_magnitude_ms, imp_surf_dist_sign_ms, with the per-sample random rotation applied to patch, sub-sample, query."""
+    imp_surf_magnitude_ms, imp_surf_dist_sign_ms, imp_surf_ms, with the per-sample random rotation applied to patch, sub-sample, query."""
     n = len(indices)
     per_shape = {}
     for pos, gi in enumerate(indices):
@@ -222,20 +222,25 @@ def _assemble_batch(dataset, indices, assembler, rng, device, dtype=torch.float3
         'imp_surf_query_point_ms': torch.matmul(q.unsqueeze(1), Rt).squeeze(1).contiguous(),
         'imp_surf_magnitude_ms': d.abs().contiguous(),
         'imp_surf_dist_sign_ms': (d >= 0).to(patch.dtype).contiguous(),        # 0.0 if sign < 0 else 1.0  (data_loader.py:367-368)
+        'imp_surf_ms': d.contiguous(),                                          # the signed distance (data_loader.py:369,402)
     }
     return {k: v.to(dtype) for k, v in batch.items()}
 
 
 def calc_metrics(pred, batch, fixed_radius=False):
-    """abs_dist_rms and the sign-classification scores of source/points_to_surf_train.py:566-598 (magnitude + sign).
-    The reference's compute_loss divides batch_data['imp_surf_magnitude_ms'] by the patch radius IN PLACE
-    (points_to_surf_train.py:552-555) before calc_metrics reads it, so the logged rmse is against the normalised target;
-    this mirror does not mutate the batch and applies the same normalisation here."""
+    """abs_dist_rms and the sign-classification scores of source/points_to_surf_train.py:566-598, for the two-output head
+    (pred [B,2]: magnitude + sign) and the regression head (pred [B,1]: signed distance).
+    The reference's compute_loss divides batch_data['imp_surf_magnitude_ms'] / ['imp_surf_ms'] by the patch radius IN
+    PLACE (points_to_surf_train.py:544-555) before calc_metrics reads it, so the logged rmse is against the normalised
+    target; for the regression head it also sets the logits to -1 / +1 in place before classifying them (:589-591), which
+    gives +1 where pred >= 0 (-0.0 included) and -1 elsewhere (NaN included).  This mirror mutates neither the batch nor
+    the logits and applies both rules here."""
     from . import evaluation
+    key = 'imp_surf_ms' if pred.shape[1] == 1 else 'imp_surf_magnitude_ms'
     abs_dist = torch.tanh(pred[:, 0]).pow(2)
-    target = batch['imp_surf_magnitude_ms'] if fixed_radius else batch['imp_surf_magnitude_ms'] / batch['patch_radius_ms']
+    target = batch[key] if fixed_radius else batch[key] / batch['patch_radius_ms']
     rms = torch.sqrt(torch.mean((abs_dist.abs() - target.abs()) ** 2))
-    inside = torch.where(pred[:, 1] >= 0.0, torch.ones_like(abs_dist), -torch.ones_like(abs_dist))
+    inside = torch.where(pred[:, -1] >= 0.0, torch.ones_like(abs_dist), -torch.ones_like(abs_dist))
     out = evaluation.compare_predictions_binary_tensors(ground_truth=batch['imp_surf_dist_sign_ms'], predicted=inside,
                                                         prediction_name='training_metrics')
     out['abs_dist_rms'] = float(rms)
@@ -305,8 +310,9 @@ def points_to_surf_train(opt, prims=None, assembler=None, device=None, dtype=tor
             except OSError:
                 print("Can't delete " + log_dirname)
 
-    output_names = [o for o in opt.outputs if o in ('imp_surf_magnitude', 'imp_surf_sign')]
-    output_loss_weights = {'imp_surf_magnitude': 1.0, 'imp_surf_sign': 1.0}
+    output_dim = arch.head_output_dim(opt.outputs)       # points_to_surf_train.py:200-240: pred_dim and the loss weights
+    output_names = [o for o in opt.outputs if o in ('imp_surf', 'imp_surf_magnitude', 'imp_surf_sign')]
+    output_loss_weights = {o: 1.0 for o in output_names}
 
     if opt.seed < 0:
         opt.seed = random.randint(1, 10000)
@@ -325,7 +331,7 @@ def points_to_surf_train(opt, prims=None, assembler=None, device=None, dtype=tor
         except ValueError:
             print(f'Warning: {opt.refine} has no epoch in the name. The log will continue at epoch 0 and might be messed up!')
     else:
-        state = initial_state_dict(opt.use_point_stn, opt.shared_transformer, opt.net_size, 2)
+        state = initial_state_dict(opt.use_point_stn, opt.shared_transformer, opt.net_size, output_dim)
 
     train_set = _ShapeSet(opt.indir, opt.trainset, opt.cache_capacity)
     test_set = _ShapeSet(opt.indir, opt.testset, opt.cache_capacity)

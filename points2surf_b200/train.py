@@ -5,8 +5,10 @@ written out by hand (there is no autograd on this path); tests compare every par
 over the reference module.
 
 Supported configuration (the hot-path subset, see points2surf_b200/eval.py:_check_supported): sym_op 'max',
-use_feat_stn 1, single_transformer 0, outputs (imp_surf_magnitude, imp_surf_sign); use_point_stn x shared_transformer in
-{(1,1) vanilla, (0,0) max, (1,0) uniform}.
+use_feat_stn 1, single_transformer 0; use_point_stn x shared_transformer in {(1,1) vanilla, (0,0) max, (1,0) uniform};
+outputs either (imp_surf_magnitude, imp_surf_sign), the two-output head, or (imp_surf,), the one-output head of the
+regression ablation (experiments/train_p2s_regression.sh), whose loss is sdf_nn.calc_loss_distance.  imp_surf together
+with magnitude / sign (the reference's three-output default) is rejected.
 
 Data parallel: one process per GPU; every rank runs the step on its shard of the batch, the flat gradient buffer is
 averaged with one all_reduce (NCCL over NVLink) and every rank applies the same update.  BatchNorm statistics stay
@@ -22,16 +24,37 @@ BN_EPS = 1e-5
 BN_MOMENTUM = 0.1
 
 
-def compute_loss(pred, batch_data, outputs, output_loss_weights, fixed_radius, prims=None, need_grad=False):
-    """Mirror of points_to_surf_train.compute_loss (:537-563) for outputs (imp_surf_magnitude, imp_surf_sign):
-    -> [loss_magnitude, loss_sign] as 0-d float64 CUDA tensors (and d(sum)/dpred when need_grad)."""
+def loss_columns(outputs):
+    """Network outputs the loss reads: 1 for (imp_surf,), 2 for (imp_surf_magnitude, imp_surf_sign); else ValueError."""
+    outputs = list(outputs)
     if 'imp_surf' in outputs:
-        raise ValueError('Unsupported output: imp_surf (regression variant); supported: imp_surf_magnitude + imp_surf_sign')
+        if 'imp_surf_magnitude' in outputs or 'imp_surf_sign' in outputs:
+            raise ValueError('Unsupported outputs %s: imp_surf (regression) together with imp_surf_magnitude / imp_surf_sign'
+                             % outputs)
+        return 1
     if not ('imp_surf_magnitude' in outputs and 'imp_surf_sign' in outputs):
-        raise ValueError('outputs must contain imp_surf_magnitude and imp_surf_sign')
+        raise ValueError('outputs must contain imp_surf_magnitude and imp_surf_sign, or imp_surf')
+    return 2
+
+
+def compute_loss(pred, batch_data, outputs, output_loss_weights, fixed_radius, prims=None, need_grad=False):
+    """Mirror of points_to_surf_train.compute_loss (:537-563): for outputs (imp_surf_magnitude, imp_surf_sign)
+    -> [loss_magnitude, loss_sign], for (imp_surf,) -> [loss_imp_surf], as 0-d float64 CUDA tensors (and
+    d(sum)/dpred [B, columns] when need_grad).  The batch is not modified (the reference divides
+    batch_data['imp_surf_ms'] / ['imp_surf_magnitude_ms'] by the radius in place; calc_metrics restates that)."""
+    cols = loss_columns(outputs)
+    if pred.dim() != 2 or pred.shape[1] != cols:
+        raise ValueError('pred %s does not match outputs %s (%d column(s))' % (tuple(pred.shape), list(outputs), cols))
     if prims is None:
         from .train_ops import CudaPrims
         prims = CudaPrims()
+    if cols == 1:
+        # sdf_nn.calc_loss_distance: mse(tanh(pred), tanh(d / r)) with the signed tanh (points_to_surf_train.py:541-548)
+        losses, dpred = prims.loss_distance(pred, batch_data['imp_surf_ms'].reshape(-1).contiguous(),
+                                            batch_data['patch_radius_ms'].reshape(-1).contiguous(),
+                                            output_loss_weights['imp_surf'], fixed_radius=fixed_radius, need_grad=need_grad)
+        out = [losses[0]]
+        return (out, dpred) if need_grad else out
     losses, dpred = prims.loss(pred, batch_data['imp_surf_magnitude_ms'].reshape(-1).contiguous(),
                                batch_data['patch_radius_ms'].reshape(-1).contiguous(),
                                batch_data['imp_surf_dist_sign_ms'].reshape(-1).contiguous(),
@@ -67,12 +90,20 @@ class TrainStep:
         self.P, self.S, self.net = int(points_per_patch), int(sub_sample_size), int(net_size)
         self.lr, self.momentum = float(lr), float(momentum)
         self.outputs = tuple(outputs)
-        self.loss_weights = output_loss_weights or {'imp_surf_magnitude': 1.0, 'imp_surf_sign': 1.0}
+        self.output_dim = loss_columns(self.outputs)
+        self.loss_weights = output_loss_weights or ({'imp_surf': 1.0} if self.output_dim == 1 else
+                                                    {'imp_surf_magnitude': 1.0, 'imp_surf_sign': 1.0})
         self.fixed_radius = bool(fixed_radius)
         sd = strip_module_prefix(state_dict)
+        if 'fc4.weight' in sd and sd['fc4.weight'].shape[0] != self.output_dim:
+            raise ValueError('the state dict has a %d-output head (fc4 %s), outputs %s need %d' % (
+                sd['fc4.weight'].shape[0], tuple(sd['fc4.weight'].shape), list(self.outputs), self.output_dim))
         some = next(iter(sd.values()))
         self.device = torch.device(device) if device is not None else some.device
-        specs = arch.layer_specs(self.use_point_stn, self.shared, self.net, 2)
+        specs = arch.layer_specs(self.use_point_stn, self.shared, self.net, self.output_dim)
+        # the batch keys the step reads (copied into the static inputs of a captured CUDA graph)
+        self._batch_keys = self._INPUT_KEYS + (('imp_surf_ms',) if self.output_dim == 1 else
+                                               ('imp_surf_magnitude_ms', 'imp_surf_dist_sign_ms'))
         # flat parameter / gradient / momentum buffers with per-tensor views (one all_reduce, one SGD launch)
         shapes = []
         for name, kind, cout, cin in specs:
@@ -216,7 +247,7 @@ class TrainStep:
 
     # ------------------------------------------------------------------------------------------ forward / backward
     def forward(self, batch):
-        """Train-mode forward -> logits [B,2]; keeps the records for backward()."""
+        """Train-mode forward -> logits [B, output_dim]; keeps the records for backward()."""
         p = self.p
         patch = batch['patch_pts_ps'].contiguous()
         B = patch.shape[0]
@@ -278,7 +309,7 @@ class TrainStep:
     def evaluate(self, batch):
         """`p2s_model.eval()` forward + compute_loss without gradients (the test batches interleaved with training,
         points_to_surf_train.py:483-500): BatchNorm uses the running statistics, nothing is recorded or updated.
-        -> (logits [B,2], [loss_magnitude, loss_sign])."""
+        -> (logits [B, output_dim], compute_loss's list: [loss_magnitude, loss_sign] or [loss_imp_surf])."""
         p = self.p
         P, S = self.P, self.S
 
@@ -347,7 +378,8 @@ class TrainStep:
 
     def step(self, batch):
         """One iteration of the reference's inner loop (points_to_surf_train.py:441-461): zero_grad, forward,
-        compute_loss, backward, SGD.  Returns [loss_magnitude, loss_sign] (0-d float64 tensors on the device)."""
+        compute_loss, backward, SGD.  Returns [loss_magnitude, loss_sign], or [loss_imp_surf] for the regression head
+        (0-d float64 tensors on the device)."""
         if self._graph is not None and self._graph_matches(batch):     # a partial last batch takes the eager step
             return self._step_graph(batch)
         logits, losses = self._forward_backward(batch)
@@ -358,8 +390,7 @@ class TrainStep:
 
     # ------------------------------------------------------------------------------------------ CUDA-graph replay
     _graph = None
-    _BATCH_KEYS = ('patch_pts_ps', 'pts_sub_sample_ms', 'imp_surf_query_point_ms', 'patch_radius_ms',
-                   'imp_surf_magnitude_ms', 'imp_surf_dist_sign_ms')
+    _INPUT_KEYS = ('patch_pts_ps', 'pts_sub_sample_ms', 'imp_surf_query_point_ms', 'patch_radius_ms')
 
     def capture_graph(self, example_batch):
         """Capture forward+backward and the SGD update of one batch shape into two CUDA graphs (the gradient all_reduce
@@ -369,7 +400,7 @@ class TrainStep:
         does not train."""
         if self.device.type != 'cuda':
             raise ValueError('CUDA graphs need a CUDA device')
-        static = {k: example_batch[k].detach().clone().contiguous() for k in self._BATCH_KEYS}
+        static = {k: example_batch[k].detach().clone().contiguous() for k in self._batch_keys}
         saved = (self.flat_params.clone(), self.flat_mom.clone(), {k: v.clone() for k, v in self.buffers.items()}, self.steps_done)
         side = torch.cuda.Stream(device=self.device)
         side.wait_stream(torch.cuda.current_stream(self.device))
@@ -410,13 +441,13 @@ class TrainStep:
 
     def _graph_matches(self, batch):
         static = self._graph[2]
-        return all(tuple(batch[k].shape) == tuple(static[k].shape) for k in self._BATCH_KEYS)
+        return all(tuple(batch[k].shape) == tuple(static[k].shape) for k in self._batch_keys)
 
     def _step_graph(self, batch):
         if (float(self.lr), float(self.momentum)) != self._graph_lr:
             self._capture_sgd()
         g1, g2, static, logits, losses = self._graph
-        for k in self._BATCH_KEYS:
+        for k in self._batch_keys:
             static[k].copy_(batch[k], non_blocking=True)
         g1.replay()
         self._reduce_gradients()

@@ -175,6 +175,21 @@ class CudaPrims:
                                        _ptr(out), _ptr(dpred) if need_grad else None, _stream()))
         return out, dpred
 
+    def loss_distance(self, pred, target, radius, w, fixed_radius=False, need_grad=True):
+        """Regression loss of the one-output head: -> (f64 [1] = [w * mse(tanh p, tanh(t / r))], dpred [B,1] or None)."""
+        pred = _f(pred, 'pred')
+        B = pred.shape[0]
+        if pred.numel() != B:
+            raise P2SError('loss_distance: pred must have one column, got %s' % (tuple(pred.shape),))
+        out = torch.empty(1, dtype=torch.float64, device=pred.device)
+        dpred = torch.empty_like(pred) if need_grad else None
+        with torch.cuda.device(pred.device):
+            check(self.lib.p2s_op_loss_distance(_ptr(pred), _ptr(_f(target, 'target')),
+                                                None if fixed_radius else _ptr(_f(radius, 'radius')), B, float(w),
+                                                1 if fixed_radius else 0, _ptr(out), _ptr(dpred) if need_grad else None,
+                                                _stream()))
+        return out, dpred
+
     def quat_to_rot(self, q):
         q = _f(q, 'q')
         R = torch.empty((q.shape[0], 3, 3), dtype=torch.float32, device=q.device)

@@ -20,8 +20,10 @@ sys.path.insert(0, os.path.join(ROOT, 'tests'))
 from points2surf_b200 import synth, ops  # noqa: E402
 from points2surf_b200.train import TrainStep  # noqa: E402
 from helpers_train import make_train_batch  # noqa: E402
+from helpers_train_regression import make_regression_train_batch  # noqa: E402
 
-FLOP_FWD = {'vanilla': 1.1407e9, 'max': 0.7768e9, 'uniform': 1.1407e9}   # SURVEY.md section 8d, per query
+# SURVEY.md section 8d, per query; 'regression' is the `uniform` network with a 128 -> 1 head (256 FLOP less per query)
+FLOP_FWD = {'vanilla': 1.1407e9, 'max': 0.7768e9, 'uniform': 1.1407e9, 'regression': 1.1407e9}
 
 
 def main():
@@ -29,7 +31,7 @@ def main():
     ap.add_argument('--batch', type=int, default=1024, help='global batch (queries per step over all ranks)')
     ap.add_argument('--steps', type=int, default=5)
     ap.add_argument('--warmup', type=int, default=2)
-    ap.add_argument('--model', default='vanilla')
+    ap.add_argument('--model', default='vanilla', help='vanilla | max | uniform | regression (one-output head, imp_surf loss)')
     ap.add_argument('--cpu_sample', type=int, default=0, help='queries of one CPU-oracle iteration timed beside it (0 = skip)')
     ap.add_argument('--graph', action='store_true', help='replay the step as CUDA graphs (TrainStep.capture_graph)')
     ap.add_argument('--profile', action='store_true', help='per-primitive time table (synchronising; slower)')
@@ -42,10 +44,13 @@ def main():
         os.environ.setdefault('MASTER_ADDR', '127.0.0.1')
         dist.init_process_group('nccl', device_id=dev)
     v = synth.VARIANTS[a.model]
+    regression = v.get('output_dim', 2) == 1
+    make_batch = make_regression_train_batch if regression else make_train_batch
+    outputs = ('imp_surf',) if regression else ('imp_surf_magnitude', 'imp_surf_sign')
     per_rank = a.batch // world
     sd = {k: t.to(dev) for k, t in synth.make_state_dict(a.model, seed=0).items()}
-    batch = {k: t.to(dev) for k, t in make_train_batch(per_rank, seed=100 + rank).items()}
-    ts = TrainStep(sd, v['use_point_stn'], v['shared_transformer'], lr=1e-4)
+    batch = {k: t.to(dev) for k, t in make_batch(per_rank, seed=100 + rank).items()}
+    ts = TrainStep(sd, v['use_point_stn'], v['shared_transformer'], lr=1e-4, outputs=outputs)
     if a.graph:
         ts.capture_graph(batch)
     prof, shapes = {}, {}
@@ -53,7 +58,7 @@ def main():
         p = ts.p
         for name in ('gemm_nt', 'gemm_tn', 'transpose', 'bn_forward', 'bn_backward', 'bn_maxpool_forward', 'bn_maxpool_backward',
                      'col_sum', 'maxpool_fwd', 'maxpool_bwd',
-                     'axpy_', 'center', 'loss', 'sgd_', 'add_row_', 'quat_to_rot', 'quat_to_rot_bwd'):
+                     'axpy_', 'center', 'loss', 'loss_distance', 'sgd_', 'add_row_', 'quat_to_rot', 'quat_to_rot_bwd'):
             fn = getattr(p, name)
 
             def wrap(fn=fn, name=name):
@@ -99,15 +104,15 @@ def main():
                'launches_per_step': ops.launch_count() / a.steps, 'cuda_graph': bool(a.graph), 'loss': [float(l) for l in losses],
                'peak_mem_GB': torch.cuda.max_memory_allocated() / 1e9}
         if a.cpu_sample > 0 and world == 1:
-            from oracle import train_oracle
-            cb = make_train_batch(a.cpu_sample, seed=100)
+            import train_regression_oracle as train_oracle
+            cb = make_batch(a.cpu_sample, seed=100)
             csd = synth.make_state_dict(a.model, seed=0)
             best = (0.0, 0)
             for th in sorted({min(os.cpu_count() or 1, c) for c in (16, 32, os.cpu_count() or 1)}):   # give the CPU arm its best thread count
                 torch.set_num_threads(th)
-                train_oracle.train_iteration(csd, cb, v['use_point_stn'], v['shared_transformer'])   # warm-up
+                train_oracle.train_iteration(csd, cb, v['use_point_stn'], v['shared_transformer'], outputs=outputs)   # warm-up
                 t0 = time.perf_counter()
-                train_oracle.train_iteration(csd, cb, v['use_point_stn'], v['shared_transformer'])
+                train_oracle.train_iteration(csd, cb, v['use_point_stn'], v['shared_transformer'], outputs=outputs)
                 rate = a.cpu_sample / (time.perf_counter() - t0)
                 if rate > best[0]:
                     best = (rate, th)
