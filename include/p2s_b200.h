@@ -392,6 +392,57 @@ typedef struct {
 int p2s_poisson_solve_dev(const float* pts, const float* normals, int64_t N, const p2s_poisson_config* cfg, float* values,
                           int64_t vcap, p2s_poisson_report* report_host, void* stream);
 
+/* ------------------------------------------------------------------ point normals --- */
+/* Oriented unit normals of an unstructured point cloud: what meshlab's "Compute normals for point sets" does before the
+ * Screened Poisson filter of the reference's normals_poisson.mlx, for clouds that come without a mesh.  Parity with
+ * meshlab / vcglib is NOT pinned: neither is part of this project, and meshlab's propagation starts at an arbitrary point
+ * without an outward seed.  The rules below are the specification (oracle/normals_oracle.py restates them on the CPU).
+ *
+ * a. Neighbours.  nbr_ids[i] = the K nearest points of the cloud to point i, point i itself included, by the float64
+ *    squared distance (dx*dx + dy*dy) + dz*dz on the fp32 coordinates with every operation rounded (p2s_knn_patch_dev's
+ *    semantics), ascending, lowest id first on ties.  3 <= K <= 64, N > K.
+ * b. Plane fit.  Float64 centroid and scatter matrix sum (p - centroid)(p - centroid)^T of the K neighbours, eigenvalues
+ *    l0 <= l1 <= l2 by cyclic Jacobi.  The fit is degenerate when !(l2 > 0) or l1 - l0 <= 1e-9 * l2 (all neighbours equal,
+ *    collinear, or isotropic): the point gets the normal (0, 0, 0) and takes no part in c.  Otherwise the normal is the
+ *    unit eigenvector of l0, rounded to fp32, with the sign that makes its component of largest magnitude positive (the
+ *    lowest axis on ties, compared on the fp32 values).
+ * c. Orientation.
+ *    P2S_NORMALS_VIEWPOINT: n is negated when n . (viewpoint - p) < 0 (float64, x then y then z, every operation rounded).
+ *    P2S_NORMALS_PROPAGATE (Hoppe et al. 1992): the graph has an edge i-j when j is among nbr_ids[i] or i among
+ *    nbr_ids[j], i != j, and both normals are non-zero.  Its cost is c = max(0, 1 - |n_i . n_j|) with
+ *    n_i . n_j = (x_i*x_j + y_i*y_j) + z_i*z_j in float64 from the fp32 normals, every operation rounded.  Edges are
+ *    totally ordered by (bits of c, min(i, j), max(i, j)), so the minimum spanning forest is unique.  Per component the
+ *    root is the point of largest z (lowest id on ties; -0 = +0) and keeps its normal when its z is > 0, is negated when
+ *    z < 0, and at z = 0 the same by y, then x.  Every other point is negated when (final normal of its forest parent) .
+ *    (its own input normal) < 0, and kept at exactly 0.  Components are oriented independently.  The result is a function
+ *    of the input alone (not of the schedule): bitwise identical across runs and streams.
+ * Both entry points synchronise `stream` (counts are read back).  Errors (non-zero return, p2s_last_error, nothing written
+ * to the outputs): NULL pointers, K outside [3, 64], N <= K, N * K >= 0x7f7f7f7f, an unknown mode, viewpoint mode without
+ * a viewpoint, non-finite coordinates, normals or viewpoint, neighbour ids outside [0, N) (the last three checked on the
+ * device before any other kernel runs). */
+#define P2S_NORMALS_PROPAGATE 0
+#define P2S_NORMALS_VIEWPOINT 1
+
+typedef struct {
+    int64_t degenerate;     /* points with a zero normal */
+    int64_t components;     /* trees of the spanning forest (propagate) */
+    int64_t flipped;        /* points whose normal was negated by c */
+    int32_t rounds;         /* Boruvka rounds that joined components */
+    int32_t sweeps;         /* level sweeps launched over the forest (a multiple of 64) */
+    float stage_ms[3];      /* CUDA-event times of a (cell index + neighbours), b, c */
+    int32_t reserved;
+} p2s_normals_stats;
+
+/* a + b + c.  pts [N,3]; viewpoint: 3 doubles on the host, NULL in propagate mode; normals_out [N,3];
+ * nbr_ids_out [N,K] int32 or NULL; stats_host or NULL. */
+int p2s_point_normals_dev(const float* pts, int64_t N, int K, int mode, const double* viewpoint, float* normals_out,
+                          int32_t* nbr_ids_out, p2s_normals_stats* stats_host, void* stream);
+/* c (propagate) alone on caller-supplied normals (unit or zero; any pre-sign) and neighbour ids [N,K], e.g. unoriented
+ * normals of another estimator.  parent_out [N] int32 or NULL: the forest parent of every point, a root's own id, -1 for a
+ * point without a normal. */
+int p2s_orient_normals_dev(const float* pts, const float* normals_in, const int32_t* nbr_ids, int64_t N, int K,
+                           float* normals_out, int32_t* parent_out, p2s_normals_stats* stats_host, void* stream);
+
 /* ------------------------------------------------------------------ training-step primitives --- */
 /* Row a14 (SURVEY.md section 8a): loss + backward + SGD of source/points_to_surf_train.py:441-461,537-563 with the
  * train-mode BatchNorm of source/points_to_surf_model.py.  Activations are row-major [rows, C] fp32.  The host side

@@ -45,7 +45,13 @@ class PoissonReport(C.Structure):
                 ('stage_ms', C.c_float * 4)]
 
 
+class NormalsStats(C.Structure):
+    _fields_ = [('degenerate', C.c_int64), ('components', C.c_int64), ('flipped', C.c_int64), ('rounds', C.c_int32),
+                ('sweeps', C.c_int32), ('stage_ms', C.c_float * 3), ('reserved', C.c_int32)]
+
+
 PRECISION_FP32, PRECISION_TC = 0, 1
+NORMALS_PROPAGATE, NORMALS_VIEWPOINT = 0, 1
 SUBSAMPLE_WEIGHTED, SUBSAMPLE_UNIFORM = 0, 1
 
 _vp, _i64, _i32, _f32 = C.c_void_p, C.c_int64, C.c_int, C.c_float
@@ -110,6 +116,9 @@ SIGNATURES = {
     'p2s_mesh_clean_dev': (C.c_int, [_vp, _i64, _vp, _i64, _vp, _i64, _vp, _i64, C.POINTER(CleanReport), _vp]),
     'p2s_poisson_solve_dev': (C.c_int, [_vp, _vp, _i64, C.POINTER(PoissonConfig), _vp, _i64, C.POINTER(PoissonReport),
                                         _vp]),
+    'p2s_point_normals_dev': (C.c_int, [_vp, _i64, _i32, _i32, C.POINTER(C.c_double), _vp, _vp, C.POINTER(NormalsStats),
+                                        _vp]),
+    'p2s_orient_normals_dev': (C.c_int, [_vp, _vp, _vp, _i64, _i32, _vp, _vp, C.POINTER(NormalsStats), _vp]),
 }
 
 _lib = None

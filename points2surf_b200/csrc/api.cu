@@ -532,6 +532,22 @@ int p2s_poisson_solve_dev(const float* pts, const float* normals, int64_t N, con
     });
 }
 
+int p2s_point_normals_dev(const float* pts, int64_t N, int K, int mode, const double* viewpoint, float* normals_out,
+                          int32_t* nbr_ids_out, p2s_normals_stats* stats_host, void* stream) {
+    return guarded([&] {
+        P2S_CHECK(pts && normals_out, "null argument");
+        point_normals(pts, N, K, mode, viewpoint, normals_out, nbr_ids_out, stats_host, as_stream(stream));
+    });
+}
+
+int p2s_orient_normals_dev(const float* pts, const float* normals_in, const int32_t* nbr_ids, int64_t N, int K,
+                           float* normals_out, int32_t* parent_out, p2s_normals_stats* stats_host, void* stream) {
+    return guarded([&] {
+        P2S_CHECK(pts && normals_in && nbr_ids && normals_out, "null argument");
+        orient_normals(pts, normals_in, nbr_ids, N, K, normals_out, parent_out, stats_host, as_stream(stream));
+    });
+}
+
 // ---- training-step primitives (train_ops.cu)
 #define P2S_OP(name, params, ...)                                   \
     int name params { return guarded([&] { __VA_ARGS__; }); }

@@ -12,15 +12,6 @@
 
 namespace p2s {
 
-// per-cloud cell index of the weighted sub-sampler (device pointers; see cloud_index_build)
-struct CloudIndex {
-    const float* meta;      // [6] bounding-box low corner, cells per unit length
-    const float* spts;      // [N,3] points in cell order
-    const int32_t* perm;    // [N]   original id of sorted point i
-    const int32_t* start;   // [C+1] first sorted point of each cell
-    const float* cbox;      // [C,6] tight bounding box of each cell's points
-};
-
 namespace {
 
 constexpr int kThreads = 256;
@@ -727,7 +718,7 @@ subsample_reject_kernel(const float* __restrict__ pts, int N, const float* __res
 // farthest corner beats the best first-point distance are scanned.  Bounds are quantised UP to multiples of 1/65535, so
 // every probability above is an exact integer ratio; 40 random bits select the slot (relative error of a point's
 // probability <= 2e-7).
-constexpr int kCG = 12, kCC = kCG * kCG * kCG;                 // 1728 cells
+constexpr int kCG = kCloudGrid, kCC = kCG * kCG * kCG;         // 1728 cells
 constexpr int kCPT = (kCC + kThreads - 1) / kThreads;          // consecutive cells per thread (7)
 
 __global__ void __launch_bounds__(1024) ci_bbox_kernel(const float* __restrict__ pts, int N, float* __restrict__ meta) {

@@ -194,6 +194,18 @@ static inline bool env_flag(const char* name) {
     return e && e[0] == '1';
 }
 
+// per-cloud cell index (device pointers): the cloud binned into kCloudGrid^3 cells of its bounding box.  Built by
+// cloud_index_build (assemble.cu) for the weighted sub-sampler; the neighbour search of normals.cu walks it too.
+constexpr int kCloudGrid = 12;
+struct CloudIndex {
+    const float* meta;      // [6] bounding-box low corner, cells per unit length
+    const float* spts;      // [N,3] points in cell order
+    const int32_t* perm;    // [N]   original id of sorted point i
+    const int32_t* start;   // [C+1] first sorted point of each cell
+    const float* cbox;      // [C,6] tight bounding box of each cell's points
+};
+const CloudIndex* cloud_index_build(const float* pts, int64_t N, cudaStream_t st);
+
 // ---- Philox4x32-10 (Salmon et al. 2011), counter-based: (key, counter) -> 4 x u32 ----
 __host__ __device__ inline void philox4x32_10(uint32_t k0, uint32_t k1, uint32_t c0, uint32_t c1,
                                               uint32_t c2, uint32_t c3, uint32_t out[4]) {

@@ -129,6 +129,11 @@ void mesh_clean(const float* verts, int64_t V, const int32_t* faces, int64_t F, 
 // poisson.cu
 void poisson_solve(const float* pts, const float* normals, int64_t N, const p2s_poisson_config& cfg, float* values,
                    int64_t cap, p2s_poisson_report* report, cudaStream_t st);
+// normals.cu
+void point_normals(const float* pts, int64_t N, int K, int mode, const double* viewpoint, float* normals_out,
+                   int32_t* nbr_ids_out, p2s_normals_stats* stats, cudaStream_t st);
+void orient_normals(const float* pts, const float* normals_in, const int32_t* nbr_ids, int64_t N, int K, float* normals_out,
+                    int32_t* parent_out, p2s_normals_stats* stats, cudaStream_t st);
 // gemm_tn_tc.cu
 bool gemm_tn_tc_ok(const float* A, int lda, const float* B, int ldb, int64_t M, int N, int K);
 void launch_gemm_tn_tc(const float* A, int lda, const float* B, int ldb, float* C, int ldc, int64_t M, int N, int K,

@@ -13,7 +13,13 @@ run; with --spsr
 
 the "SPSR + GT normals" stage of eval_dataset.py:143-158 runs instead, with the reconstruction on the GPU
 (apply_meshlab_filter, points2surf_b200/poisson.py): 06_normals, then 06_poisson_rec_gt_normals/<name>.ply, then
-comp_poisson_rec_gt_normals.csv against 03_meshes for the shapes in valset.txt."""
+comp_poisson_rec_gt_normals.csv against 03_meshes for the shapes in valset.txt.  With --spsr_estimated_normals
+
+    python -m points2surf_b200.eval_dataset DATASET_DIR --spsr_estimated_normals
+
+the stage of the reference's normals_poisson.mlx (eval_dataset.py:160-172) runs without meshlab and without meshes: oriented
+normals estimated from 04_pts alone (ops.point_normals) into 06_normals_est, Screened Poisson from them into 06_poisson_rec,
+and comp_poisson_rec_ml_normals.csv when 03_meshes and valset.txt exist."""
 import argparse
 import os
 import sys
@@ -32,6 +38,8 @@ from . import sdf
 
 # the Screened Poisson parameters of the reference's poisson.mlx that this reconstruction uses
 POISSON_MLX_DEFAULTS = dict(depth=8, point_weight=4.0, scale=1.1, iters=8)
+# the "Compute normals for point sets" parameters of the reference's normals_poisson.mlx
+NORMALS_MLX_DEFAULTS = dict(k=10, smooth_iter=0, flip_flag=False, view_pos=(0.0, 0.0, 0.0))
 _MLX_PARAMS = dict(depth=('depth', int), pointWeight=('point_weight', float), scale=('scale', float),
                    iters=('iters', int))
 
@@ -119,6 +127,11 @@ def apply_meshlab_filter(base_dir, dataset_dir, pts_dir, recon_mesh_dir, num_pro
     else from poisson.mlx (POISSON_MLX_DEFAULTS).  `num_processes` and `meshlabserver_bin` are accepted and ignored."""
     params = read_poisson_filter(filter_file) if filter_file and os.path.isfile(filter_file) \
         else dict(POISSON_MLX_DEFAULTS)
+    _poisson_reconstruct_dir(base_dir, dataset_dir, pts_dir, recon_mesh_dir, params)
+
+
+def _poisson_reconstruct_dir(base_dir, dataset_dir, pts_dir, recon_mesh_dir, params):
+    """The per-file loop of apply_meshlab_filter with the Screened Poisson parameters given."""
     pts_dir_abs = os.path.join(base_dir, dataset_dir, pts_dir)
     recon_mesh_dir_abs = os.path.join(base_dir, dataset_dir, recon_mesh_dir)
     os.makedirs(recon_mesh_dir_abs, exist_ok=True)
@@ -136,6 +149,84 @@ def apply_meshlab_filter(base_dir, dataset_dir, pts_dir, recon_mesh_dir, num_pro
         mesh_io.write_ply(mesh_abs, verts, faces)
 
 
+def read_normals_poisson_filter(filter_file):
+    """A meshlab filter script of the shape of the reference's normals_poisson.mlx: "Compute normals for point sets", then
+    Screened Poisson ("Delete Current Mesh" filters are ignored).
+    -> (dict(k, smooth_iter, flip_flag, view_pos), Screened Poisson parameters like read_poisson_filter's).
+    Raises ValueError for any other script, and for smoothIter != 0 (normal smoothing is not built)."""
+    normals = dict(NORMALS_MLX_DEFAULTS)
+    params = dict(POISSON_MLX_DEFAULTS)
+    filters = [e for e in ET.parse(filter_file).getroot() if e.tag in ('filter', 'xmlfilter')
+               and 'delete current mesh' not in e.get('name', '').lower()]
+    names = [e.get('name', '') for e in filters]
+    if len(filters) != 2 or 'compute normals for point sets' not in names[0].lower() \
+            or 'screened poisson' not in names[1].lower():
+        raise ValueError('{}: expected "Compute normals for point sets" followed by Screened Poisson, found {}'.format(
+            filter_file, names))
+    for p in filters[0]:
+        name = p.get('name')
+        if name == 'K':
+            normals['k'] = int(p.get('value'))
+        elif name == 'smoothIter':
+            normals['smooth_iter'] = int(p.get('value'))
+        elif name == 'flipFlag':
+            normals['flip_flag'] = p.get('value', '').lower() == 'true'
+        elif name == 'viewPos':
+            normals['view_pos'] = tuple(float(p.get(a)) for a in ('x', 'y', 'z'))
+    if normals['smooth_iter'] != 0:
+        raise ValueError('{}: smoothIter = {} (normal smoothing is not built)'.format(filter_file, normals['smooth_iter']))
+    for p in filters[1]:
+        if p.get('name') in _MLX_PARAMS:
+            key, conv = _MLX_PARAMS[p.get('name')]
+            params[key] = conv(p.get('value'))
+    return normals, params
+
+
+def estimate_pts_normals(base_dir, dataset_dir, dir_in_pointcloud, dir_out_normals, k=10, flip_flag=False,
+                         view_pos=(0.0, 0.0, 0.0)):
+    """For every <name>.xyz.npy in dir_in_pointcloud ([N,3] or [N,6]; the points are columns 0:3) write the estimated
+    oriented normals dir_out_normals/<name>.xyz.npy (float64 [N,3], like 06_normals) and dir_out_normals/pts/<name>.xyz,
+    unless both are newer than the input.  ops.point_normals over k neighbours; flip_flag: every normal faces view_pos
+    (meshlab's flipFlag / viewPos), else the signs are propagated over the cloud."""
+    dir_in_abs = os.path.join(base_dir, dataset_dir, dir_in_pointcloud)
+    dir_out_abs = os.path.join(base_dir, dataset_dir, dir_out_normals)
+    dir_out_pts_abs = os.path.join(dir_out_abs, 'pts')
+    os.makedirs(dir_out_pts_abs, exist_ok=True)
+    dev = sdf._device()
+    for f in sorted(f for f in os.listdir(dir_in_abs) if os.path.isfile(os.path.join(dir_in_abs, f)) and f[-4:] == '.npy'):
+        pts_in = os.path.join(dir_in_abs, f)
+        normals_out = os.path.join(dir_out_abs, f)
+        pts_normals_out = os.path.join(dir_out_pts_abs, f[:-8] + '.xyz')
+        if not sdf._call_necessary([pts_in], [normals_out, pts_normals_out]):
+            continue
+        pts = np.load(pts_in)[:, :3]
+        p = torch.from_numpy(np.ascontiguousarray(pts, np.float32)).to(dev)
+        normals = ops.point_normals(p, k=k, mode='viewpoint' if flip_flag else 'propagate',
+                                    viewpoint=view_pos if flip_flag else None).cpu().numpy().astype(np.float64)
+        np.save(normals_out, normals)
+        point_cloud.write_xyz(pts_normals_out, pts, normals=normals)
+
+
+def _spsr_estimated_normals(dataset, base_dir, dataset_dir):
+    """The normals_poisson.mlx stage of eval_dataset.py:160-172 without meshlab: 06_normals_est, 06_poisson_rec and, when
+    03_meshes and valset.txt exist, comp_poisson_rec_ml_normals.csv."""
+    filter_file = 'normals_poisson.mlx'
+    normals, params = read_normals_poisson_filter(filter_file) if os.path.isfile(filter_file) \
+        else (dict(NORMALS_MLX_DEFAULTS), dict(POISSON_MLX_DEFAULTS))
+    print('### normal estimation for point cloud')
+    estimate_pts_normals(base_dir=base_dir, dataset_dir=dataset_dir, dir_in_pointcloud='04_pts',
+                         dir_out_normals='06_normals_est', k=normals['k'], flip_flag=normals['flip_flag'],
+                         view_pos=normals['view_pos'])
+    print('### poisson reconstruction from estimated normals')
+    _poisson_reconstruct_dir(base_dir, dataset_dir, '06_normals_est/pts', '06_poisson_rec', params)
+    if os.path.isdir(os.path.join(dataset, '03_meshes')) and os.path.isfile(os.path.join(dataset, 'valset.txt')):
+        print('### normal estimation and poisson reconstruction - hausdorff distance')
+        evaluation.mesh_comparison(new_meshes_dir_abs=os.path.join(dataset, '06_poisson_rec'),
+                                   ref_meshes_dir_abs=os.path.join(dataset, '03_meshes'), num_processes=1,
+                                   report_name=os.path.join(dataset, 'comp_poisson_rec_ml_normals.csv'),
+                                   samples_per_model=10000, dataset_file_abs=os.path.join(dataset, 'valset.txt'))
+
+
 def main(argv=None):
     parser = argparse.ArgumentParser(description='Ground-truth point normals (06_normals) for the point clouds in '
                                                  'DATASET_DIR/04_pts from the meshes in DATASET_DIR/03_meshes.')
@@ -144,9 +235,17 @@ def main(argv=None):
                         help='also reconstruct Screened Poisson surfaces from the ground-truth normals on the GPU '
                              '(06_poisson_rec_gt_normals) and compare them with 03_meshes for the shapes in valset.txt '
                              '(comp_poisson_rec_gt_normals.csv)')
+    parser.add_argument('--spsr_estimated_normals', action='store_true',
+                        help='estimate oriented normals from 04_pts alone on the GPU (06_normals_est), reconstruct Screened '
+                             'Poisson surfaces from them (06_poisson_rec) and, when 03_meshes and valset.txt exist, compare '
+                             '(comp_poisson_rec_ml_normals.csv); needs neither 03_meshes nor 06_normals')
     args = parser.parse_args(argv)
     dataset = os.path.abspath(args.dataset_dir)
     base_dir, dataset_dir = os.path.dirname(dataset), os.path.basename(dataset)
+    if args.spsr_estimated_normals:
+        _spsr_estimated_normals(dataset, base_dir, dataset_dir)
+        if not args.spsr:
+            return
     if args.spsr:
         print('### Screened-Poisson reconstruction from PCPNet normals (06_poisson_rec_pcpnet_normals) needs '
               'PCPNet\'s normals: skipped')

@@ -385,6 +385,56 @@ def poisson_solve(pts, normals, depth=8, point_weight=4.0, scale=1.1, iters=8):
     return values, report
 
 
+def _normals_stats(st):
+    return dict(degenerate=st.degenerate, components=st.components, flipped=st.flipped, rounds=st.rounds, sweeps=st.sweeps,
+                stage_ms=list(st.stage_ms))
+
+
+def point_normals(pts, k=10, mode='propagate', viewpoint=None, return_neighbours=False, return_stats=False):
+    """Oriented unit normals [N,3] fp32 of the cloud pts [N,3] (rules in include/p2s_b200.h, "point normals"): plane fit
+    over the k nearest points, then mode 'propagate' (signs along the minimum spanning forest of the kNN graph, each
+    component's highest point facing up) or 'viewpoint' (every normal faces `viewpoint`).  A point whose fit is degenerate
+    gets (0, 0, 0).  Optionally also the neighbour ids [N,k] int32 and the stats dict of p2s_normals_stats."""
+    pts = _dev(pts, torch.float32, 'pts')
+    if pts.dim() != 2 or pts.shape[1] != 3:
+        raise P2SError('pts must have shape [N, 3]')
+    if mode not in ('propagate', 'viewpoint'):
+        raise ValueError("mode must be 'propagate' or 'viewpoint', got %r" % (mode,))
+    if mode == 'viewpoint' and viewpoint is None:
+        raise ValueError("mode 'viewpoint' needs a viewpoint")
+    N, k = pts.shape[0], int(k)
+    vp = (C.c_double * 3)(*[float(x) for x in viewpoint]) if viewpoint is not None else None
+    normals = torch.empty((N, 3), dtype=torch.float32, device=pts.device)
+    ids = torch.empty((N, max(k, 0)), dtype=torch.int32, device=pts.device) if return_neighbours else None
+    st = _lib.NormalsStats()
+    with torch.cuda.device(pts.device):
+        check(_lib.load().p2s_point_normals_dev(
+            _ptr(pts), N, k, _lib.NORMALS_VIEWPOINT if mode == 'viewpoint' else _lib.NORMALS_PROPAGATE, vp, _ptr(normals),
+            _ptr(ids) if ids is not None else None, C.byref(st), _stream()))
+    out = (normals,) + ((ids,) if return_neighbours else ()) + ((_normals_stats(st),) if return_stats else ())
+    return out if len(out) > 1 else normals
+
+
+def orient_normals(pts, normals, nbr_ids, return_parents=False, return_stats=False):
+    """The 'propagate' orientation of point_normals alone, on caller-supplied normals [N,3] fp32 (unit, or zero for a point
+    to leave out) and neighbour ids [N,k] int32.  -> oriented normals, optionally the forest parent of every point [N]
+    int32 (a root's own id, -1 without a normal) and the stats dict."""
+    pts = _dev(pts, torch.float32, 'pts')
+    nrm = _dev(normals, torch.float32, 'normals')
+    ids = _dev(nbr_ids, torch.int32, 'nbr_ids')
+    if pts.dim() != 2 or pts.shape[1] != 3 or nrm.shape != pts.shape or ids.dim() != 2 or ids.shape[0] != pts.shape[0]:
+        raise P2SError('pts and normals must have shape [N, 3] and nbr_ids [N, k]')
+    N = pts.shape[0]
+    out = torch.empty((N, 3), dtype=torch.float32, device=pts.device)
+    parents = torch.empty((N,), dtype=torch.int32, device=pts.device) if return_parents else None
+    st = _lib.NormalsStats()
+    with torch.cuda.device(pts.device):
+        check(_lib.load().p2s_orient_normals_dev(_ptr(pts), _ptr(nrm), _ptr(ids), N, ids.shape[1], _ptr(out),
+                                                 _ptr(parents) if parents is not None else None, C.byref(st), _stream()))
+    res = (out,) + ((parents,) if return_parents else ()) + ((_normals_stats(st),) if return_stats else ())
+    return res if len(res) > 1 else out
+
+
 SCANNER_DEFAULTS = dict(res_x=176, res_y=144, lens_angle_w=43.6, lens_angle_h=34.6, max_distance=10.0, noise_mu=0.0)
 
 
