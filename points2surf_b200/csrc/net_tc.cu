@@ -10,12 +10,12 @@
 // transform into conv1's weights per query (W1*T), both exactly as in the fp32 path up to operation order.
 //
 // Tile = 64 points of one query (segments are padded with a duplicate of their first point: max-invariant).
-// Mid layers: M = 64 points, A operand = activations in registers (the accumulator fragment of one layer, packed to
-// fp16 pairs, is the A fragment of the next), B operand = weights in smem.  Big layer 128 -> 1024: M = 64 channels,
-// A = resident W3 block in smem, B = the tile's 128-channel activations in smem, D[channel][point] so that the max
-// over points is a per-thread reduction over accumulator columns (the 4 lanes sharing a row are combined once per
-// query).  Each CTA owns 512 of the 1024 channels (its half of W3, 128 KB fp16, stays resident in shared memory);
-// CTA 2j and 2j+1 stream the same queries.
+// Every layer after the first: M = 64 points, A operand = activations in registers (the accumulator fragment of one
+// layer, packed to fp16 pairs, is the A fragment of the next), B operand = weights in smem.  The big layer 128 -> 1024
+// runs as m64n128 per 128-channel chunk with B = the resident W3 chunk, so the activations never go through shared
+// memory; D[point][channel], and the max over points is a max over accumulator rows (in-thread, then a shuffle
+// reduce-scatter across the warp, then across the 4 warps once per query).  Each CTA owns 512 of the 1024 channels
+// (its half of W3, 128 KB fp16, stays resident in shared memory); CTA 2j and 2j+1 stream the same queries.
 //
 // Each warpgroup of the CTA streams its own queries (qi = wg, wg + 2, ...) through all layers; the two warpgroups
 // interleave on the SM, so one's FMA / epilogue work overlaps the other's tensor-core work.
@@ -30,32 +30,32 @@ using namespace ptx;
 
 namespace {
 
-constexpr int kTile = 64;                       // points per tile (M of the mid layers, N of the big layer)
+constexpr int kTile = 64;                       // points per tile (M of every tensor-core layer)
 constexpr int kWG = 2;                          // warpgroups per CTA
 constexpr int kThreads = 128 * kWG;
-constexpr uint32_t kAct2Bytes = kTile * 128 * 2;   // 64 points x 128 channels fp16
 // shared memory map (bytes).  PRECISE = split-precision variant used for the guard-band recompute: every fp16
 // operand x is carried as x_hi + x_lo and every product is evaluated as a_hi*b_hi + a_lo*b_hi + a_hi*b_lo (three MMAs
-// per k-step, ~2^-22 relative), so the images are twice as large and a CTA owns one 128-channel chunk instead of four.
+// per k-step, ~2^-22 relative), so the images are twice as large and a CTA owns two 128-channel chunks instead of four.
 template <bool PRECISE>
 struct Cfg {
-    static constexpr int kChunks = PRECISE ? 1 : 4;                  // 128-channel chunks of the big layer per CTA
+    static constexpr int kChunks = PRECISE ? 2 : 4;                  // 128-channel chunks of the big layer per CTA
     static constexpr int kSplit = 8 / kChunks;                       // CTAs that share one query stream
     static constexpr uint32_t kChunkBytes = PRECISE ? 65536u : 32768u;   // W3 chunk image (hi [+ lo])
     static constexpr uint32_t kW3Bytes = kChunks * kChunkBytes;
     static constexpr uint32_t kMidScale = PRECISE ? 2u : 1u;
     static constexpr uint32_t kMidBytes = (8192u + 8192u + 16384u) * kMidScale;
     static constexpr uint32_t kPerqBytes = PRECISE ? 16384u : 8192u; // per-query conv1*(T+I) image
+    static constexpr uint32_t kRedBytes = 4u * kChunks * 128u * 4u;  // end of query: [warp][channel] maxima, aliases perq
     static constexpr uint32_t kOffMid = kW3Bytes;
-    // per warpgroup: the big layer's B operand (hi [| lo]), the per-query conv1 image, (W0*R)^T [3][64] fp32
-    static constexpr uint32_t kWgPerq = kAct2Bytes * kMidScale;
-    static constexpr uint32_t kWgWq = kWgPerq + kPerqBytes;
+    // per warpgroup: the per-query conv1 image, (W0*R)^T [3][64] fp32
+    static constexpr uint32_t kWgWq = kPerqBytes;
     static constexpr uint32_t kWgBytes = kWgWq + 192 * 4;
     static constexpr uint32_t kOffWg = kOffMid + kMidBytes;
     static constexpr uint32_t kOffBias = kOffWg + kWG * kWgBytes;     // [256] mid biases back to back, [64] first-layer bias
     static constexpr uint32_t kSmemBytes = kOffBias + 320 * 4;
 };
 static_assert(Cfg<false>::kSmemBytes <= 232448 && Cfg<true>::kSmemBytes <= 232448, "shared memory budget");
+static_assert(Cfg<false>::kRedBytes <= Cfg<false>::kPerqBytes && Cfg<true>::kRedBytes <= Cfg<true>::kPerqBytes, "reduction scratch");
 
 struct Seg {
     const float* ptr;   // [B, n, 3]
@@ -114,6 +114,29 @@ __device__ __forceinline__ void mid_mma(float (&d)[R], const uint32_t (&a)[4], c
     }
 }
 
+// epilogue of a mid layer: m64nN accumulator + bias, ReLU, fp16 pairs -> the A fragments of the next layer's N/16 k-steps
+template <bool PRECISE, int R, int KL>
+__device__ __forceinline__ void pack_acc(const float (&d)[R], const float* bias, int q4, uint32_t (&a)[R / 8][4], uint32_t (&al)[R / 8][KL]) {
+#pragma unroll
+    for (int j = 0; j < R / 4; ++j) {
+        const float2 bb = *reinterpret_cast<const float2*>(bias + 8 * j + 2 * q4);
+        pack_act<PRECISE>(d[4 * j] + bb.x, d[4 * j + 1] + bb.y, a[j >> 1][(j & 1) * 2], al[j >> 1][PRECISE ? (j & 1) * 2 : 0]);
+        pack_act<PRECISE>(d[4 * j + 2] + bb.x, d[4 * j + 3] + bb.y, a[j >> 1][(j & 1) * 2 + 1], al[j >> 1][PRECISE ? (j & 1) * 2 + 1 : 0]);
+    }
+}
+
+// one step of a butterfly max reduce-scatter between lanes l and l ^ S: each keeps m[0 .. S) for the half of m[0 .. 2S)
+// selected by its lane bit S, folded with the partner's values of that half
+template <int S>
+__device__ __forceinline__ void max_halve(float (&m)[32], int lane) {
+    const bool up = (lane & S) != 0;
+#pragma unroll
+    for (int i = 0; i < S; ++i) {
+        const float send = up ? m[i] : m[i + S], keep = up ? m[i + S] : m[i];
+        m[i] = fmaxf(keep, __shfl_xor_sync(0xffffffffu, send, S));
+    }
+}
+
 template <bool PRECISE>
 __global__ void __launch_bounds__(kThreads, 1) pointnet_pass_kernel(const PassParams p) {
     using C = Cfg<PRECISE>;
@@ -156,14 +179,13 @@ __global__ void __launch_bounds__(kThreads, 1) pointnet_pass_kernel(const PassPa
     __syncthreads();
 
     uint8_t* wsm = smem + C::kOffWg + wg * C::kWgBytes;
-    uint8_t* act2 = wsm;                                                  // [point][channel] K-major, LBO 128, SBO 2048
-    uint8_t* perq = wsm + C::kWgPerq;
+    uint8_t* perq = wsm;
+    float* red = reinterpret_cast<float*>(perq);                          // [4 warps][kChunks * 128 channels]
     float* wq = reinterpret_cast<float*>(wsm + C::kWgWq);                 // [3][64]: rows of (W0*R)^T
     const float* s_b0 = s_bias + 256;
     const uint32_t bar_id = 1 + (uint32_t)wg;
     auto wg_sync = [&]() { asm volatile("bar.sync %0, 128;" ::"r"(bar_id) : "memory"); };
-    const uint64_t dsc_act2 = make_smem_desc(smem_u32(act2), 128, 2048);
-    const uint64_t dsc_w3 = make_smem_desc(smem_u32(smem), 128, 2048);
+    const uint64_t dsc_w3 = make_smem_desc(smem_u32(smem), 128, 2048);   // N = 128 channels of a chunk, K-major
     uint64_t dsc_mid[3], dsc_mid_lo[3];
     for (int l = 0; l < 3; ++l) {
         const bool pq = l == p.perq_layer;
@@ -193,9 +215,10 @@ __global__ void __launch_bounds__(kThreads, 1) pointnet_pass_kernel(const PassPa
             fence_proxy_async_smem();
         }
         wg_sync();
-        float rmax[4 * C::kChunks];                   // [chunk][64-channel block][row r0 | r0 + 8]
+        // [chunk][i]: max over the warp's 16 points so far of chunk channel 16 (lane / 4) + 8 (i / 2) + 2 q4 + i % 2
+        float vmax[4 * C::kChunks];
 #pragma unroll
-        for (int i = 0; i < 4 * C::kChunks; ++i) rmax[i] = -INFINITY;
+        for (int i = 0; i < 4 * C::kChunks; ++i) vmax[i] = -INFINITY;
         for (int tq = 0; tq < tpq; ++tq) {
             // ---- first layer (fp32 FMA): points r0, r0 + 8 of the tile, channels 16 kk + 8 hc + 2 q4 + {0, 1}
             const int sgi = tq < p.seg[0].tiles ? 0 : 1;
@@ -229,102 +252,105 @@ __global__ void __launch_bounds__(kThreads, 1) pointnet_pass_kernel(const PassPa
                     }
                 }
             }
-            // ---- mid layers: 64 -> 64 (A stays in registers), the last one 64 -> 128 (into the big layer's B operand)
-            int boff = 0;
-            for (int l = 0; l < p.num_mid; ++l) {
-                const float* bl = s_bias + boff;
-                const uint64_t w = dsc_mid[l], w_lo = dsc_mid_lo[l];
-                if (l < p.num_mid - 1) {
-                    float d[32];
+            // ---- mid layers: 64 -> 64 ..., then 64 -> 128 into the big layer's A fragments; A stays in registers
+            const float* bl = s_bias;
 #pragma unroll
-                    for (int i = 0; i < 32; ++i) d[i] = 0.f;
-                    wgmma_fence();
+            for (int l = 0; l < 2; ++l) {
+                if (l >= p.num_mid - 1) break;
+                float d[32];
 #pragma unroll
-                    for (int ks = 0; ks < 4; ++ks)
-                        mid_mma<PRECISE>(d, a[ks], reinterpret_cast<const uint32_t (&)[4]>(al[PRECISE ? ks : 0]), w + (uint64_t)(ks * 16), w_lo + (uint64_t)(ks * 16), ks > 0);
-                    wgmma_commit();
-                    wgmma_wait<0>();
-                    fence_regs(d);
+                for (int i = 0; i < 32; ++i) d[i] = 0.f;
+                wgmma_fence();
 #pragma unroll
-                    for (int j = 0; j < 8; ++j) {
-                        const float2 bb = *reinterpret_cast<const float2*>(bl + 8 * j + 2 * q4);
-                        pack_act<PRECISE>(d[4 * j] + bb.x, d[4 * j + 1] + bb.y, a[j >> 1][(j & 1) * 2], al[j >> 1][PRECISE ? (j & 1) * 2 : 0]);
-                        pack_act<PRECISE>(d[4 * j + 2] + bb.x, d[4 * j + 3] + bb.y, a[j >> 1][(j & 1) * 2 + 1], al[j >> 1][PRECISE ? (j & 1) * 2 + 1 : 0]);
-                    }
-                } else {
-                    float d[64];
-#pragma unroll
-                    for (int i = 0; i < 64; ++i) d[i] = 0.f;
-                    wgmma_fence();
-#pragma unroll
-                    for (int ks = 0; ks < 4; ++ks)
-                        mid_mma<PRECISE>(d, a[ks], reinterpret_cast<const uint32_t (&)[4]>(al[PRECISE ? ks : 0]), w + (uint64_t)(ks * 16), w_lo + (uint64_t)(ks * 16), ks > 0);
-                    wgmma_commit();
-                    wgmma_wait<0>();
-                    fence_regs(d);
-                    wg_sync();                            // the previous tile's big-layer MMAs have read act2
-#pragma unroll
-                    for (int j = 0; j < 16; ++j) {
-                        const int k = 8 * j + 2 * q4;
-                        const float2 bb = *reinterpret_cast<const float2*>(bl + k);
-#pragma unroll
-                        for (int h = 0; h < 2; ++h) {
-                            const int pt = r0 + 8 * h;
-                            const uint32_t off = (uint32_t)(pt >> 3) * 2048u + (uint32_t)j * 128u + (uint32_t)(pt & 7) * 16u + (uint32_t)q4 * 4u;
-                            uint32_t hi, lo = 0;
-                            pack_act<PRECISE>(d[4 * j + 2 * h] + bb.x, d[4 * j + 2 * h + 1] + bb.y, hi, lo);
-                            *reinterpret_cast<uint32_t*>(act2 + off) = hi;
-                            if (PRECISE) *reinterpret_cast<uint32_t*>(act2 + kAct2Bytes + off) = lo;
-                        }
-                    }
-                    fence_proxy_async_smem();
-                    wg_sync();
-                }
-                boff += p.mid_N[l];
+                for (int ks = 0; ks < 4; ++ks)
+                    mid_mma<PRECISE>(d, a[ks], reinterpret_cast<const uint32_t (&)[4]>(al[PRECISE ? ks : 0]), dsc_mid[l] + (uint64_t)(ks * 16), dsc_mid_lo[l] + (uint64_t)(ks * 16), ks > 0);
+                wgmma_commit();
+                wgmma_wait<0>();
+                fence_regs(d);
+                pack_acc<PRECISE>(d, bl, q4, a, al);
+                bl += 64;
             }
-            // ---- big layer 128 -> this CTA's channels: D[64 channels][64 points] per block, max over the points
+            uint32_t a2[8][4], a2l[8][kL];                // the tile's 128 activations: A fragments of the big layer's 8 k-steps
+            {
+                const uint64_t w = p.num_mid == 3 ? dsc_mid[2] : dsc_mid[0], w_lo = p.num_mid == 3 ? dsc_mid_lo[2] : dsc_mid_lo[0];
+                float d[64];
 #pragma unroll
+                for (int i = 0; i < 64; ++i) d[i] = 0.f;
+                wgmma_fence();
+#pragma unroll
+                for (int ks = 0; ks < 4; ++ks)
+                    mid_mma<PRECISE>(d, a[ks], reinterpret_cast<const uint32_t (&)[4]>(al[PRECISE ? ks : 0]), w + (uint64_t)(ks * 16), w_lo + (uint64_t)(ks * 16), ks > 0);
+                wgmma_commit();
+                wgmma_wait<0>();
+                fence_regs(d);
+                pack_acc<PRECISE>(d, bl, q4, a2, a2l);
+            }
+            // ---- big layer 128 -> this CTA's channels: D[64 points][128 channels] per chunk, max over the points.  Unrolled,
+            // ptxas overlaps one chunk's reduction with the next chunk's MMAs (two accumulators); the precise variant's
+            // twice-as-large A fragments leave no registers for that, so its loop stays rolled.  vmax[0 .. 4) is always the
+            // current chunk's: the running maxima rotate by one chunk per iteration, back in order after the last one.
+#pragma unroll(PRECISE ? 1 : C::kChunks)
             for (int c = 0; c < C::kChunks; ++c) {
-                float d0[32], d1[32];
+                float d[64];
 #pragma unroll
-                for (int i = 0; i < 32; ++i) { d0[i] = 0.f; d1[i] = 0.f; }
-                const uint64_t wa = dsc_w3 + (uint64_t)((uint32_t)c * (C::kChunkBytes >> 4)), wb = wa + (uint64_t)(16384u >> 4);
+                for (int i = 0; i < 64; ++i) d[i] = 0.f;
+                const uint64_t w = dsc_w3 + (uint64_t)((uint32_t)c * (C::kChunkBytes >> 4));
                 wgmma_fence();
 #pragma unroll
                 for (int ks = 0; ks < 8; ++ks) {
-                    const uint64_t x = dsc_act2 + (uint64_t)(ks * 16), o = (uint64_t)(ks * 16);
-                    if (PRECISE) {
-                        const uint64_t x_lo = x + (uint64_t)(kAct2Bytes >> 4), lo = (uint64_t)(32768u >> 4);
-                        wgmma_ss_n64(d0, wa + lo + o, x, ks > 0); wgmma_ss_n64(d0, wa + o, x_lo, 1); wgmma_ss_n64(d0, wa + o, x, 1);
-                        wgmma_ss_n64(d1, wb + lo + o, x, ks > 0); wgmma_ss_n64(d1, wb + o, x_lo, 1); wgmma_ss_n64(d1, wb + o, x, 1);
+                    const uint64_t o = w + (uint64_t)(ks * 16);
+                    if (PRECISE) {                        // small terms first: a_hi*w_lo, a_lo*w_hi, then a_hi*w_hi
+                        wgmma_rs_n128(d, a2[ks], o + (uint64_t)(32768u >> 4), ks > 0);
+                        wgmma_rs_n128(d, reinterpret_cast<const uint32_t (&)[4]>(a2l[PRECISE ? ks : 0]), o, 1);
+                        wgmma_rs_n128(d, a2[ks], o, 1);
                     } else {
-                        wgmma_ss_n64(d0, wa + o, x, ks > 0);
-                        wgmma_ss_n64(d1, wb + o, x, ks > 0);
+                        wgmma_rs_n128(d, a2[ks], o, ks > 0);
                     }
                 }
                 wgmma_commit();
                 wgmma_wait<0>();
-                fence_regs(d0);
-                fence_regs(d1);
+                fence_regs(d);
+                // rows r0, r0 + 8 in-thread, then a reduce-scatter over the 8 lanes of a column group (lane bits 2-4): at
+                // each step a lane keeps half of its values and receives its partner's maxima of that half; what is left,
+                // m[i] for i < 4, is element 4 (lane / 4) + i of the original 32
+                float m[32];
 #pragma unroll
-                for (int j = 0; j < 8; ++j) {
-                    rmax[4 * c + 0] = fmaxf(rmax[4 * c + 0], fmaxf(d0[4 * j], d0[4 * j + 1]));
-                    rmax[4 * c + 1] = fmaxf(rmax[4 * c + 1], fmaxf(d0[4 * j + 2], d0[4 * j + 3]));
-                    rmax[4 * c + 2] = fmaxf(rmax[4 * c + 2], fmaxf(d1[4 * j], d1[4 * j + 1]));
-                    rmax[4 * c + 3] = fmaxf(rmax[4 * c + 3], fmaxf(d1[4 * j + 2], d1[4 * j + 3]));
+                for (int j = 0; j < 16; ++j) {
+                    m[2 * j] = fmaxf(d[4 * j], d[4 * j + 2]);
+                    m[2 * j + 1] = fmaxf(d[4 * j + 1], d[4 * j + 3]);
                 }
+                max_halve<16>(m, lane);
+                max_halve<8>(m, lane);
+                max_halve<4>(m, lane);
+                float v[4];
+#pragma unroll
+                for (int i = 0; i < 4; ++i) v[i] = fmaxf(vmax[i], m[i]);
+#pragma unroll
+                for (int i = 0; i < 4 * (C::kChunks - 1); ++i) vmax[i] = vmax[i + 4];
+#pragma unroll
+                for (int i = 0; i < 4; ++i) vmax[4 * (C::kChunks - 1) + i] = v[i];
             }
         }
-        // ---- the 4 lanes of a row hold disjoint point columns: combine, then one lane writes the channel
+        // ---- combine the 4 warps through shared memory (perq is dead: every MMA of this query has completed), then one
+        // thread per 4 consecutive channels writes them
+        constexpr int kC = C::kChunks * 128;
+        const int warp = t >> 5;
+        wg_sync();
 #pragma unroll
-        for (int i = 0; i < 4 * C::kChunks; ++i) {
-            rmax[i] = fmaxf(rmax[i], __shfl_xor_sync(0xffffffffu, rmax[i], 1));
-            rmax[i] = fmaxf(rmax[i], __shfl_xor_sync(0xffffffffu, rmax[i], 2));
-        }
-        if (q4 == 0) {
+        for (int c = 0; c < C::kChunks; ++c)
 #pragma unroll
-            for (int i = 0; i < 4 * C::kChunks; ++i)
-                p.out[q * 1024 + (size_t)((part * C::kChunks + (i >> 2)) * 128 + ((i >> 1) & 1) * 64 + r0 + (i & 1) * 8)] = rmax[i];
+            for (int h = 0; h < 2; ++h)
+                *reinterpret_cast<float2*>(red + warp * kC + c * 128 + 16 * (lane >> 2) + 8 * h + 2 * q4) = make_float2(vmax[4 * c + 2 * h], vmax[4 * c + 2 * h + 1]);
+        wg_sync();
+        for (int i = t; i < kC / 4; i += 128) {
+            const float4* r4 = reinterpret_cast<const float4*>(red);
+            float4 v = r4[i];
+#pragma unroll
+            for (int w = 1; w < 4; ++w) {
+                const float4 u = r4[w * (kC / 4) + i];
+                v = make_float4(fmaxf(v.x, u.x), fmaxf(v.y, u.y), fmaxf(v.z, u.z), fmaxf(v.w, u.w));
+            }
+            *reinterpret_cast<float4*>(p.out + q * 1024 + (size_t)(part * kC + 4 * i)) = v;
         }
     }
 }
