@@ -50,10 +50,12 @@ void p2s_launch_count_reset(void);
 typedef struct p2s_model p2s_model;
 
 /* Mirrors the constructor arguments of source/points_to_surf_model.py:238-240 as used by
- * source/points_to_surf_eval.py:150-166.  Supported subset (SURVEY.md section 8b): sym_op='max',
- * single_transformer=0, use_feat_stn=1.  The head's output_dim is not part of this struct: the functions without
- * the _ex suffix mean output_dim=2 (imp_surf_magnitude, imp_surf_sign); the _ex variants also take output_dim=1, the
- * regression head of the imp_surf ablation (experiments/train_p2s_regression.sh). */
+ * source/points_to_surf_eval.py:150-166.  Supported subset (SURVEY.md section 8b): sym_op='max', use_feat_stn=1.
+ * The head's output_dim and single_transformer are not part of this struct: the functions without a suffix mean
+ * output_dim=2 (imp_surf_magnitude, imp_surf_sign) and single_transformer=0; the _ex variants also take output_dim=1, the
+ * regression head of the imp_surf ablation (experiments/train_p2s_regression.sh); the _enc variants also take
+ * single_transformer=1, the shared-encoder ablation (experiments/train_p2s_shared_encoder.sh), which requires
+ * use_point_stn=1 and shared_transformer=0. */
 typedef struct {
     int32_t use_point_stn;      /* train_opt.use_point_stn                                  */
     int32_t shared_transformer; /* train_opt.shared_transformer                             */
@@ -71,10 +73,16 @@ typedef struct {
  *   blob := [STN3(point_stn) if use_point_stn && shared_transformer]
  *           FEAT(feat_local, 0)  FEAT(feat_global, use_point_stn && !shared_transformer)
  *           fc1_local fc1_global fc2 fc3 fc4            (fc4: 128 -> output_dim)
+ * and with single_transformer=1 (one PointNetfeat over cat(patch, sub-sample - q), points_to_surf_model.py:253-263):
+ *   blob := FEAT(feat_local_global, 1)  fc1_local_global  fc2 fc3 fc4
+ *           (fc1_local_global: 1024 -> 1024 with bn1_local_global folded; fc2: 1024 -> 256 as above)
  * points2surf_b200/weights.py builds it from a reference state_dict. */
 size_t p2s_model_blob_floats(const p2s_model_config* cfg);
 /* the same for a head of output_dim outputs (1 or 2); 0 for any other output_dim */
 size_t p2s_model_blob_floats_ex(const p2s_model_config* cfg, int output_dim);
+/* the same for single_transformer 0 or 1; 0 for an unsupported combination (single_transformer=1 needs use_point_stn=1
+ * and shared_transformer=0).  p2s_model_blob_floats_ex(cfg, d) == p2s_model_blob_floats_enc(cfg, d, 0). */
+size_t p2s_model_blob_floats_enc(const p2s_model_config* cfg, int output_dim, int single_transformer);
 
 /* Replaces make_regressor (source/points_to_surf_eval.py:150-171): builds the device-resident,
  * kernel-ready weight set on CUDA device `device`. */
@@ -83,6 +91,12 @@ int p2s_model_create(const p2s_model_config* cfg, const float* blob_host, size_t
 /* output_dim 2: p2s_model_create.  output_dim 1: the regression head (outputs imp_surf).  Any other value is an error. */
 int p2s_model_create_ex(const p2s_model_config* cfg, int output_dim, const float* blob_host, size_t blob_floats,
                         int device, p2s_model** out);
+/* single_transformer 0: p2s_model_create_ex.  1: the shared encoder; the configuration is checked (use_point_stn=1,
+ * shared_transformer=0) before any device work, and anything else is an error with a message.  Both engines run it:
+ * the tensor-core path as three passes over both segments (QSTN -> R; STN64 with R; final stack with R and the per-query
+ * conv1 * (T + I) image), then fc1_local_global, fc2, fc3, fc4. */
+int p2s_model_create_enc(const p2s_model_config* cfg, int output_dim, int single_transformer, const float* blob_host,
+                         size_t blob_floats, int device, p2s_model** out);
 void p2s_model_destroy(p2s_model* m);
 
 /* Arithmetic of the per-point MLP stacks:
@@ -106,7 +120,8 @@ int p2s_profile_get(p2s_model* m, double* ms, int64_t* launches, double* flops);
 
 /* Diagnostic tap used by the parity tests: when `aux` (device, [B][P2S_AUX_STRIDE] floats) is non-NULL every
  * following forward also writes, per query, the point rotation R (9), feat_local's max feature (1024) and
- * feat_global's max feature (1024) -- trans / the PointNetfeat outputs of points_to_surf_model.py:326-343. */
+ * feat_global's max feature (1024) -- trans / the PointNetfeat outputs of points_to_surf_model.py:326-343.  For a
+ * single_transformer model: R (9), feat_local_global's max feature (1024, conv3 bias included), then 1024 zeros. */
 #define P2S_AUX_STRIDE 2064
 int p2s_model_set_debug_aux(p2s_model* m, float* aux);
 

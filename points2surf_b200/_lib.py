@@ -65,6 +65,8 @@ SIGNATURES = {
     'p2s_model_create': (C.c_int, [C.POINTER(ModelConfig), _vp, C.c_size_t, C.c_int, C.POINTER(_vp)]),
     'p2s_model_blob_floats_ex': (C.c_size_t, [C.POINTER(ModelConfig), C.c_int]),
     'p2s_model_create_ex': (C.c_int, [C.POINTER(ModelConfig), C.c_int, _vp, C.c_size_t, C.c_int, C.POINTER(_vp)]),
+    'p2s_model_blob_floats_enc': (C.c_size_t, [C.POINTER(ModelConfig), C.c_int, C.c_int]),
+    'p2s_model_create_enc': (C.c_int, [C.POINTER(ModelConfig), C.c_int, C.c_int, _vp, C.c_size_t, C.c_int, C.POINTER(_vp)]),
     'p2s_model_destroy': (None, [_vp]),
     'p2s_model_set_precision': (C.c_int, [_vp, C.c_int, _f32]),
     'p2s_model_last_guard_count': (C.c_int, [_vp, C.POINTER(_i64)]),

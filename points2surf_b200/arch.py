@@ -19,8 +19,11 @@ def head_output_dim(outputs):
     return 2
 
 
-def layer_specs(use_point_stn, shared_transformation, net=1024, output_dim=2):
-    """-> list of (dotted name, kind in {'conv','fc','bn'}, cout, cin) in state_dict order."""
+def layer_specs(use_point_stn, shared_transformation, net=1024, output_dim=2, single_transformer=False):
+    """-> list of (dotted name, kind in {'conv','fc','bn'}, cout, cin) in state_dict order.
+    single_transformer: the shared encoder (source/points_to_surf_model.py:253-263): feat_local_global (its QSTN iff
+    use_point_stn), fc1_local_global (net -> net), bn1_local_global, then the common head; shared_transformation plays
+    no part."""
 
     def stn(prefix, dim, quat):
         out = 4 if quat else dim * dim
@@ -44,12 +47,16 @@ def layer_specs(use_point_stn, shared_transformation, net=1024, output_dim=2):
         return s
 
     specs = []
-    if use_point_stn and shared_transformation:
-        specs += stn('point_stn.', 3, True)
-    specs += feat('feat_local.', False)
-    specs += feat('feat_global.', bool(use_point_stn and not shared_transformation))
-    specs += [('fc1_local', 'fc', net // 2, net), ('fc1_global', 'fc', net // 2, net),
-              ('bn1_local', 'bn', net // 2, 0), ('bn1_global', 'bn', net // 2, 0),
-              ('fc2', 'fc', net // 4, net), ('fc3', 'fc', net // 8, net // 4), ('fc4', 'fc', output_dim, net // 8),
+    if single_transformer:
+        specs += feat('feat_local_global.', bool(use_point_stn))
+        specs += [('fc1_local_global', 'fc', net, net), ('bn1_local_global', 'bn', net, 0)]
+    else:
+        if use_point_stn and shared_transformation:
+            specs += stn('point_stn.', 3, True)
+        specs += feat('feat_local.', False)
+        specs += feat('feat_global.', bool(use_point_stn and not shared_transformation))
+        specs += [('fc1_local', 'fc', net // 2, net), ('fc1_global', 'fc', net // 2, net),
+                  ('bn1_local', 'bn', net // 2, 0), ('bn1_global', 'bn', net // 2, 0)]
+    specs += [('fc2', 'fc', net // 4, net), ('fc3', 'fc', net // 8, net // 4), ('fc4', 'fc', output_dim, net // 8),
               ('bn2', 'bn', net // 4, 0), ('bn3', 'bn', net // 8, 0)]
     return specs

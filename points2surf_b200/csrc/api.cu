@@ -82,9 +82,11 @@ size_t feat_floats(bool qstn, int net) {
     auto l = [](size_t co, size_t ci) { return co * ci + co; };
     return (qstn ? stn_floats(3, 4, net) : 0) + stn_floats(64, 4096, net) + l(64, 3) + l(64, 64) + l(64, 64) + l(128, 64) + l(net, 128);
 }
-size_t blob_floats(const p2s_model_config& c, int output_dim) {
+size_t blob_floats(const p2s_model_config& c, int output_dim, int single_transformer) {
     auto l = [](size_t co, size_t ci) { return co * ci + co; };
     const int net = c.net_size;
+    if (single_transformer)   // FEAT(feat_local_global, 1) fc1_local_global fc2 fc3 fc4
+        return feat_floats(true, net) + l(net, net) + l(net / 4, net) + l(net / 8, net / 4) + l(output_dim, net / 8);
     const bool shared = c.use_point_stn && c.shared_transformer;
     const bool gq = c.use_point_stn && !c.shared_transformer;
     return (shared ? stn_floats(3, 4, net) : 0) + feat_floats(false, net) + feat_floats(gq, net) +
@@ -98,6 +100,15 @@ void check_cfg(const p2s_model_config& c) {
 }
 
 bool output_dim_ok(int output_dim) { return output_dim == 1 || output_dim == 2; }
+
+// the shared encoder exists as the published ablation only (experiments/train_p2s_shared_encoder.sh): its own QSTN
+// (use_point_stn 1) and no shared point_stn (shared_transformer 0); -> null if the combination is supported, else why not
+const char* single_transformer_error(const p2s_model_config& c, int single_transformer) {
+    if (single_transformer != 0 && single_transformer != 1) return "single_transformer must be 0 or 1";
+    if (single_transformer && c.use_point_stn != 1) return "single_transformer=1 needs use_point_stn=1 (the encoder's own QSTN)";
+    if (single_transformer && c.shared_transformer != 0) return "single_transformer=1 needs shared_transformer=0";
+    return nullptr;
+}
 
 cudaStream_t as_stream(void* s) { return reinterpret_cast<cudaStream_t>(s); }
 
@@ -221,8 +232,12 @@ size_t p2s_model_blob_floats(const p2s_model_config* cfg) {
 }
 
 size_t p2s_model_blob_floats_ex(const p2s_model_config* cfg, int output_dim) {
-    if (!cfg || !output_dim_ok(output_dim)) return 0;
-    return blob_floats(*cfg, output_dim);
+    return p2s_model_blob_floats_enc(cfg, output_dim, 0);
+}
+
+size_t p2s_model_blob_floats_enc(const p2s_model_config* cfg, int output_dim, int single_transformer) {
+    if (!cfg || !output_dim_ok(output_dim) || single_transformer_error(*cfg, single_transformer)) return 0;
+    return blob_floats(*cfg, output_dim, single_transformer);
 }
 
 int p2s_model_create(const p2s_model_config* cfg, const float* blob_host, size_t n_floats, int device, p2s_model** out) {
@@ -231,11 +246,18 @@ int p2s_model_create(const p2s_model_config* cfg, const float* blob_host, size_t
 
 int p2s_model_create_ex(const p2s_model_config* cfg, int output_dim, const float* blob_host, size_t n_floats, int device,
                         p2s_model** out) {
+    return p2s_model_create_enc(cfg, output_dim, 0, blob_host, n_floats, device, out);
+}
+
+int p2s_model_create_enc(const p2s_model_config* cfg, int output_dim, int single_transformer, const float* blob_host,
+                         size_t n_floats, int device, p2s_model** out) {
     return guarded([&] {
         P2S_CHECK(cfg && blob_host && out, "null argument");
         check_cfg(*cfg);
         P2S_CHECK(output_dim_ok(output_dim), "output_dim must be 1 (imp_surf) or 2 (imp_surf_magnitude, imp_surf_sign)");
-        P2S_CHECK(n_floats == blob_floats(*cfg, output_dim), "weight blob size does not match the model config");
+        const char* enc_err = single_transformer_error(*cfg, single_transformer);
+        P2S_CHECK(!enc_err, enc_err);
+        P2S_CHECK(n_floats == blob_floats(*cfg, output_dim, single_transformer), "weight blob size does not match the model config");
         int ndev = 0;
         cudaError_t e = cudaGetDeviceCount(&ndev);
         if (e != cudaSuccess || ndev == 0) throw Error("no CUDA device available: libp2s_b200 has no CPU fallback");
@@ -255,12 +277,18 @@ int p2s_model_create_ex(const p2s_model_config* cfg, int output_dim, const float
         P2S_CUDA(cudaMemset(m->guard_count_dev, 0, sizeof(int64_t)));
         BlobCursor c{m->blob, n_floats};
         const int net = cfg->net_size;
-        m->shared_qstn = cfg->use_point_stn && cfg->shared_transformer;
-        if (m->shared_qstn) m->point_stn = take_stn(c, 3, 4, net);
-        m->local = take_feat(c, false, net);
-        m->global = take_feat(c, cfg->use_point_stn && !cfg->shared_transformer, net);
-        m->fc1_local = c.take(net / 2, net);
-        m->fc1_global = c.take(net / 2, net);
+        if (single_transformer) {
+            m->single_transformer = true;
+            m->enc = take_feat(c, true, net);
+            m->fc1_enc = c.take(net, net);
+        } else {
+            m->shared_qstn = cfg->use_point_stn && cfg->shared_transformer;
+            if (m->shared_qstn) m->point_stn = take_stn(c, 3, 4, net);
+            m->local = take_feat(c, false, net);
+            m->global = take_feat(c, cfg->use_point_stn && !cfg->shared_transformer, net);
+            m->fc1_local = c.take(net / 2, net);
+            m->fc1_global = c.take(net / 2, net);
+        }
         m->fc2 = c.take(net / 4, net);
         m->fc3 = c.take(net / 8, net / 4);
         m->fc4 = c.take(output_dim, net / 8);

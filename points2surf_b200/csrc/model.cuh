@@ -31,6 +31,12 @@ struct Model {
     Stn point_stn;
     Feat local, global;
     Layer fc1_local, fc1_global, fc2, fc3, fc4;
+    // shared-encoder ablation (single_transformer=1, points_to_surf_model.py:253-263,320-323): one PointNetfeat with its
+    // own QSTN over cat(patch, sub-sample - q) replaces point_stn / local / global, fc1_enc (1024 -> 1024) replaces
+    // fc1_local / fc1_global; those stay empty
+    bool single_transformer = false;
+    Feat enc;                            // feat_local_global
+    Layer fc1_enc;                       // fc1_local_global, bn1_local_global folded
 
     int precision = P2S_PRECISION_FP32;
     float guard_band = 0.f;
@@ -50,9 +56,11 @@ struct Model {
     int* guard_list_count = nullptr;
     int64_t guard_list_cap = 0;
     int64_t guard_base = 0;
-    float* debug_aux = nullptr;          // optional [B][kAuxStride]: R(9), feat_local_max(1024), feat_global_max(1024)
+    float* debug_aux = nullptr;          // optional [B][kAuxStride]: R(9), feat_local_max(1024), feat_global_max(1024);
+                                         // shared encoder: R(9), feat_local_global's max(1024), 1024 zeros
 };
 constexpr int kAuxStride = 2064;
+// fg may be null (shared encoder): its 1024 slots are written as zeros
 void debug_aux_copy(Model& m, int64_t b0, int64_t Bc, const float* R, const float* fl, const float* fg, cudaStream_t st);
 
 // net_fp32.cu

@@ -280,7 +280,7 @@ __global__ void debug_aux_kernel(float* aux, int64_t b0, int64_t Bc, const float
     float v = 0.f;
     if (j < 9) v = R ? R[b * 9 + j] : (j % 4 == 0 ? 1.f : 0.f);
     else if (j < 9 + 1024) v = fl[b * 1024 + (j - 9)];
-    else if (j < 9 + 2048) v = fg[b * 1024 + (j - 9 - 1024)];
+    else if (j < 9 + 2048) v = fg ? fg[b * 1024 + (j - 9 - 1024)] : 0.f;
     aux[(b0 + b) * kAuxStride + j] = v;
 }
 void debug_aux_copy(Model& m, int64_t b0, int64_t Bc, const float* R, const float* fl, const float* fg, cudaStream_t st) {
@@ -437,6 +437,25 @@ void forward_fp32(Model& m, const float* patch, const float* sub, const float* q
         const float* su = sub + b0 * S * 3;
         const float* qu = query + b0 * 3;
         const float* R_local = nullptr;
+        if (m.single_transformer) {
+            // shared encoder (model.py:320-323): x = cat(patch, shape - q); feat_local_global's QSTN sees and rotates all
+            // P + S points (model.py:180-184); the rotated points go to bufB, which feat() reads only in its first layer,
+            // before its STN64 reuses the buffer
+            transform_points(pa, nullptr, nullptr, w.xall, Bc, P, PS, 0, st);
+            transform_points(su, qu, nullptr, w.xall, Bc, S, PS, P, st);
+            stn(m.enc.stn1, w.xall, Bc, PS, w, w.q4, st);
+            launch_quat_to_rot(w.q4, w.R, Bc, st);
+            transform_points(pa, nullptr, w.R, w.bufB, Bc, P, PS, 0, st);
+            transform_points(su, qu, w.R, w.bufB, Bc, S, PS, P, st);
+            float* fmax = w.fb_local;
+            feat(m.enc, w.bufB, Bc, PS, w, fmax, st);
+            debug_aux_copy(m, b0, Bc, w.R, fmax, nullptr, st);
+            fc(m.fc1_enc, fmax, w.cat, Bc, true, st);                  // fc1_local_global + bn + ReLU (model.py:323)
+            fc(m.fc2, w.cat, w.h3, Bc, true, st);
+            fc(m.fc3, w.h3, w.h4, Bc, true, st);
+            fc(m.fc4, w.h4, logits + b0 * m.fc4.cout, Bc, false, st);
+            continue;
+        }
         if (m.shared_qstn) {
             // feats = cat(patch, shape - q); trans = QSTN(feats)   (model.py:303,325-331)
             transform_points(pa, nullptr, nullptr, w.xall, Bc, P, PS, 0, st);

@@ -497,13 +497,19 @@ struct TcFc {                 // one Linear layer: fp32 weights + (optional) ten
 struct TcStnFc { TcFc fc1, fc2, fc3; };
 
 struct TcWeights {
-    TcStack qstn;                // pass A
+    TcStack qstn;                // pass A (point_stn, feat_global.stn1 or feat_local_global.stn1)
     TcStack stn[2], fin[2];      // [0] local, [1] global: pass B, pass C
     TcStnFc qstn_fc, stn_fc[2];
     TcFc head_fc1[2], head_fc2, head_fc3;
     // conv1 folded into stn2.fc3 per branch: images of G [4096 x 256] and bias g0 [4096]
     const uint8_t* fold_img[2] = {nullptr, nullptr};
     const float* fold_bias[2] = {nullptr, nullptr};
+    // shared encoder (feat_local_global): passes B and C, the STN64 tail and its fold, fc1_local_global
+    TcStack stn_enc, fin_enc;
+    TcStnFc stn_fc_enc;
+    TcFc head_fc1_enc;
+    const uint8_t* fold_img_enc = nullptr;
+    const float* fold_bias_enc = nullptr;
     bool fc_on_tc = true;
     std::vector<void*> allocs;
     int sm_count = 132;
@@ -665,19 +671,33 @@ void tc_build(Model& m) {
         return f;
     };
     auto mk_stn_fc = [&](const Stn& s) { TcStnFc r; r.fc1 = mk_fc(s.fc1); r.fc2 = mk_fc(s.fc2); r.fc3 = mk_fc(s.fc3); return r; };
-    if (m.shared_qstn) t->qstn_fc = mk_stn_fc(m.point_stn);
-    else if (m.global.has_qstn) t->qstn_fc = mk_stn_fc(m.global.stn1);
-    t->stn_fc[0] = mk_stn_fc(m.local.stn2);
-    t->stn_fc[1] = mk_stn_fc(m.global.stn2);
-    for (int br = 0; br < 2; ++br) {
-        const Feat& f = br ? m.global : m.local;
+    auto fold = [&](const Feat& f, const uint8_t*& img, const float*& bias) {
         P2S_CHECK(f.stn2.fc3.cout == 4096 && f.stn2.fc3.cin == 256 && f.conv1.cout == 64 && f.conv1.cin == 64, "unexpected STN shape");
         float* G = reinterpret_cast<float*>(tc_alloc(*t, (size_t)4096 * 256 * 4));
         float* g0 = reinterpret_cast<float*>(tc_alloc(*t, 4096 * 4));
         P2S_LAUNCH(fold_fc3_kernel, 4096, 256, 0, 0, f.conv1.W, f.stn2.fc3.W, f.stn2.fc3.b, G, g0);
-        t->fold_img[br] = fc_tc_pack_raw(G, 4096, 256, t->allocs);
-        t->fold_bias[br] = g0;
+        img = fc_tc_pack_raw(G, 4096, 256, t->allocs);
+        bias = g0;
+    };
+    if (m.single_transformer) {
+        // one encoder over patch + sub-sample: only its stacks exist (local / global / point_stn are empty)
+        t->qstn_fc = mk_stn_fc(m.enc.stn1);
+        t->stn_fc_enc = mk_stn_fc(m.enc.stn2);
+        fold(m.enc, t->fold_img_enc, t->fold_bias_enc);
+        t->head_fc1_enc = mk_fc(m.fc1_enc);
+        t->head_fc2 = mk_fc(m.fc2);
+        t->head_fc3 = mk_fc(m.fc3);
+        build_stn(t->qstn, m.enc.stn1, nullptr, nullptr);
+        build_stn(t->stn_enc, m.enc.stn2, &m.enc.conv0a, &m.enc.conv0b);
+        build_fin(t->fin_enc, m.enc);
+        P2S_CUDA(cudaDeviceSynchronize());
+        return;
     }
+    if (m.shared_qstn) t->qstn_fc = mk_stn_fc(m.point_stn);
+    else if (m.global.has_qstn) t->qstn_fc = mk_stn_fc(m.global.stn1);
+    t->stn_fc[0] = mk_stn_fc(m.local.stn2);
+    t->stn_fc[1] = mk_stn_fc(m.global.stn2);
+    for (int br = 0; br < 2; ++br) fold(br ? m.global : m.local, t->fold_img[br], t->fold_bias[br]);
     t->head_fc1[0] = mk_fc(m.fc1_local);
     t->head_fc1[1] = mk_fc(m.fc1_global);
     t->head_fc2 = mk_fc(m.fc2);
@@ -748,6 +768,34 @@ static void forward_tc_core(Model& m, const float* patch, const float* sub, cons
         if (out_f2) launch_fc_tc_img(imgB, f.fc2.img, f.fc2.L->b, out_f2, 256, Bc, 256, 512, true, st, 0);
         else launch_fc_tc_img(imgB, f.fc2.img, f.fc2.L->b, imgC, 0, Bc, 256, 512, true, st, 3, 8, 0);
     };
+    // tail of a pass A (QSTN): raw max gmax -> fc1, fc2, fc3 -> quaternion q4 -> rotation R
+    auto qstn_rot = [&](const Layer& c3, int64_t Bc) {
+        { StageScope ts("net: fc tails", st);
+          if (fc_tc && img_ok(t.qstn_fc)) {
+              stn_tail_img(c3, t.qstn_fc, gmax, Bc, f2);
+              run_fc(t.qstn_fc.fc3, f2, 256, q4, 4, Bc, false, false, st);
+          } else fc_tail(c3, t.qstn_fc, fc_tc, gmax, Bc, g, f1, f2, q4, st); }
+        launch_quat_to_rot(q4, R, Bc, st);
+    };
+    // tail of a pass B (STN64 of feature stack f): raw max gmax -> the per-query operand image of conv1 * (T + I) in perq
+    auto stn64_perq = [&](const Feat& f, const TcStnFc& fc, const uint8_t* fold_img, const float* fold_bias, int64_t Bc) {
+        if (fc_tc) {
+            // fc1, fc2, then the folded last layer writes the per-query fp16 operand images of conv1*(T+I) directly
+            StageScope ts("net: fc tails", st);
+            if (img_ok(fc)) {
+                stn_tail_img(f.stn2.c3, fc, gmax, Bc, nullptr);
+                launch_fc_tc_img(imgC, fold_img, fold_bias, perq, 0, Bc, 4096, 256, false, st, precise ? 2 : 1);
+            } else {
+                run_fc(fc.fc1, gmax, 1024, f1, 512, Bc, true, true, st, f.stn2.c3.b, true);
+                run_fc(fc.fc2, f1, 512, f2, 256, Bc, true, true, st);
+                launch_fc_tc(f2, 256, fold_img, fold_bias, reinterpret_cast<float*>(perq), 0, Bc, 4096, 256, false, st, precise ? 2 : 1);
+            }
+        } else {
+            { StageScope ts("net: fc tails", st); fc_tail(f.stn2.c3, fc, false, gmax, Bc, g, f1, f2, T, st); }
+            // W1' = conv1.W * (T + I) -> per-query fp16 operand images (one fused kernel)
+            { StageScope ts("net: fold W1*T", st); P2S_LAUNCH(fold_w1_kernel, (unsigned)Bc, 256, 0, st, f.conv1.W, T, Bc, perq); }
+        }
+    };
 
     for (int64_t b0 = 0; b0 < B; b0 += Bc_max) {
         const int64_t Bc = (B - b0 < Bc_max) ? (B - b0) : Bc_max;
@@ -755,23 +803,46 @@ static void forward_tc_core(Model& m, const float* patch, const float* sub, cons
         const float* su = sub + b0 * S * 3;
         const float* qu = query + b0 * 3;
         const float* Rq = nullptr;
+        if (m.single_transformer) {
+            // shared encoder (model.py:320-323): every pass runs over both segments, cat(patch, sub - q), so each pass still
+            // sees P + S points per query, but there are three passes instead of five and one STN64 tail instead of two
+            const Seg sp = make_seg(pa, P, 0), ss = make_seg(su, S, 1);
+            // pass A: feat_local_global.stn1 -> R, which rotates all P + S points (model.py:180-184)
+            { StageScope ts("net: pass kernels", st); launch_pass(m, t.qstn, sp, ss, qu, nullptr, Bc, -1, nullptr, gmax, st, precise); }
+            qstn_rot(m.enc.stn1.c3, Bc);
+            // pass B: STN64 over both segments with R folded into W0 -> the per-query conv1 * (T + I) image
+            { StageScope ts("net: pass kernels", st); launch_pass(m, t.stn_enc, sp, ss, qu, R, Bc, -1, nullptr, gmax, st, precise); }
+            stn64_perq(m.enc, t.stn_fc_enc, t.fold_img_enc, t.fold_bias_enc, Bc);
+            // pass C: both segments with R and the per-query image -> the encoder's raw max feature
+            { StageScope ts("net: pass kernels", st); launch_pass(m, t.fin_enc, sp, ss, qu, R, Bc, 1, perq, fmax_l, st, precise); }
+            const bool fuse_b3 = fc_tc && !m.debug_aux && t.head_fc1_enc.img;
+            if (!fuse_b3) launch_bias_act(fmax_l, m.enc.conv3.b, Bc, 1024, false, st);
+            debug_aux_copy(m, b0, Bc, R, fmax_l, nullptr, st);
+            StageScope ts_head("net: fc tails", st);
+            if (fuse_b3 && t.head_fc2.img && t.head_fc3.img) {
+                // fc1_local_global (N = 1024) writes fc2's K = 1024 operand image directly
+                uint8_t* imgCat = reinterpret_cast<uint8_t*>(cat);
+                launch_pack_a(fmax_l, 1024, Bc, 1024, m.enc.conv3.b, false, imgA, st);
+                launch_fc_tc_img(imgA, t.head_fc1_enc.img, m.fc1_enc.b, imgCat, 0, Bc, 1024, 1024, true, st, 3, 32, 0);
+                launch_fc_tc_img(imgCat, t.head_fc2.img, m.fc2.b, imgC, 0, Bc, 256, 1024, true, st, 3, 8, 0);
+                launch_fc_tc_img(imgC, t.head_fc3.img, m.fc3.b, h4, 128, Bc, 128, 256, true, st, 0);
+            } else {
+                run_fc(t.head_fc1_enc, fmax_l, 1024, cat, 1024, Bc, true, fc_tc, st, fuse_b3 ? m.enc.conv3.b : nullptr, false);
+                run_fc(t.head_fc2, cat, 1024, h3, 256, Bc, true, fc_tc, st);
+                run_fc(t.head_fc3, h3, 256, h4, 128, Bc, true, fc_tc, st);
+            }
+            const int od = m.fc4.cout;
+            launch_gemm_nt(h4, 0, 128, m.fc4.W, 0, m.fc4.b, logits + b0 * od, 0, od, (int)Bc, od, 128, 1, false, st);
+            continue;
+        }
         if (m.shared_qstn) {
             // pass A over cat(patch, sub - q)   (model.py:303,325-327)
             { StageScope ts("net: pass kernels", st); launch_pass(m, t.qstn, make_seg(pa, P, 0), make_seg(su, S, 1), qu, nullptr, Bc, -1, nullptr, gmax, st, precise); }
-            { StageScope ts("net: fc tails", st);
-              if (fc_tc && img_ok(t.qstn_fc)) {
-                  stn_tail_img(m.point_stn.c3, t.qstn_fc, gmax, Bc, f2);
-                  run_fc(t.qstn_fc.fc3, f2, 256, q4, 4, Bc, false, false, st);
-              } else fc_tail(m.point_stn.c3, t.qstn_fc, fc_tc, gmax, Bc, g, f1, f2, q4, st); }
-            launch_quat_to_rot(q4, R, Bc, st);
+            qstn_rot(m.point_stn.c3, Bc);
             Rq = R;
         } else if (m.global.has_qstn) {
             launch_pass(m, t.qstn, make_seg(su, S, 1), make_seg(nullptr, 0, 0), qu, nullptr, Bc, -1, nullptr, gmax, st, precise);
-            if (fc_tc && img_ok(t.qstn_fc)) {
-                stn_tail_img(m.global.stn1.c3, t.qstn_fc, gmax, Bc, f2);
-                run_fc(t.qstn_fc.fc3, f2, 256, q4, 4, Bc, false, false, st);
-            } else fc_tail(m.global.stn1.c3, t.qstn_fc, fc_tc, gmax, Bc, g, f1, f2, q4, st);
-            launch_quat_to_rot(q4, R, Bc, st);
+            qstn_rot(m.global.stn1.c3, Bc);
             Rq = R;
         }
         for (int br = 1; br >= 0; --br) {    // global first like the reference, then local
@@ -780,22 +851,7 @@ static void forward_tc_core(Model& m, const float* patch, const float* sub, cons
             float* fmax = br ? fmax_g : fmax_l;
             // pass B: STN64 -> T
             { StageScope ts("net: pass kernels", st); launch_pass(m, t.stn[br], sg, make_seg(nullptr, 0, 0), qu, Rq, Bc, -1, nullptr, gmax, st, precise); }
-            if (fc_tc) {
-                // fc1, fc2, then the folded last layer writes the per-query fp16 operand images of conv1*(T+I) directly
-                StageScope ts("net: fc tails", st);
-                if (img_ok(t.stn_fc[br])) {
-                    stn_tail_img(f.stn2.c3, t.stn_fc[br], gmax, Bc, nullptr);
-                    launch_fc_tc_img(imgC, t.fold_img[br], t.fold_bias[br], perq, 0, Bc, 4096, 256, false, st, precise ? 2 : 1);
-                } else {
-                    run_fc(t.stn_fc[br].fc1, gmax, 1024, f1, 512, Bc, true, true, st, f.stn2.c3.b, true);
-                    run_fc(t.stn_fc[br].fc2, f1, 512, f2, 256, Bc, true, true, st);
-                    launch_fc_tc(f2, 256, t.fold_img[br], t.fold_bias[br], reinterpret_cast<float*>(perq), 0, Bc, 4096, 256, false, st, precise ? 2 : 1);
-                }
-            } else {
-                { StageScope ts("net: fc tails", st); fc_tail(f.stn2.c3, t.stn_fc[br], false, gmax, Bc, g, f1, f2, T, st); }
-                // W1' = conv1.W * (T + I) -> per-query fp16 operand images (one fused kernel)
-                { StageScope ts("net: fold W1*T", st); P2S_LAUNCH(fold_w1_kernel, (unsigned)Bc, 256, 0, st, f.conv1.W, T, Bc, perq); }
-            }
+            stn64_perq(f, t.stn_fc[br], t.fold_img[br], t.fold_bias[br], Bc);
             (void)Tt;
             // pass C: final stack -> max feature (bias, no ReLU: model.py:203,210-212)
             { StageScope ts("net: pass kernels", st); launch_pass(m, t.fin[br], sg, make_seg(nullptr, 0, 0), qu, Rq, Bc, 1, perq, fmax, st, precise); }

@@ -73,12 +73,23 @@ def _output_dim(train_opt):
     return 1 if 'imp_surf' in train_opt.outputs else 2
 
 
+def _single_transformer(train_opt):
+    return bool(getattr(train_opt, 'single_transformer', 0))
+
+
 def _check_supported(train_opt, eval_opt):
-    arch.head_output_dim(train_opt.outputs)
+    output_dim = arch.head_output_dim(train_opt.outputs)
     if getattr(train_opt, 'sym_op', 'max') != 'max':
         raise ValueError('Unsupported symmetric operation: %s' % train_opt.sym_op)
-    if getattr(train_opt, 'single_transformer', 0):
-        raise ValueError('Unsupported option: single_transformer=1')
+    if _single_transformer(train_opt):
+        # the shared-encoder ablation as experiments/train_p2s_shared_encoder.sh trains it: its own QSTN and the
+        # magnitude + sign head.  The reference reads use_point_stn unconditionally (points_to_surf_eval.py:157), so a
+        # params file without it fails there as well.
+        if not getattr(train_opt, 'use_point_stn', 0):
+            raise ValueError('Unsupported option: single_transformer=1 without use_point_stn=1')
+        if output_dim != 2:
+            raise ValueError('Unsupported option: single_transformer=1 with outputs %s (only imp_surf_magnitude + '
+                             'imp_surf_sign)' % list(train_opt.outputs))
     if getattr(train_opt, 'fixed_subsample', 0) and not getattr(train_opt, 'uniform_subsample', 0):
         raise ValueError('Unsupported option: fixed_subsample=1 with the distance-weighted sub-sample (only with uniform_subsample=1)')
     if eval_opt.sampling not in ('full', 'sequential_shapes_random_patches'):
@@ -199,11 +210,13 @@ def points_to_surf_eval(eval_opt):
         train_opt = _load_train_opt(param_filename)
         _check_supported(train_opt, eval_opt)
         state = strip_module_prefix(torch.load(model_filename, map_location='cpu'))
-        eng = ops.Engine(state, train_opt.use_point_stn, train_opt.shared_transformer,
+        single = _single_transformer(train_opt)
+        # the shared encoder ignores shared_transformer (points_to_surf_model.py:253-263)
+        eng = ops.Engine(state, train_opt.use_point_stn, 0 if single else train_opt.shared_transformer,
                          points_per_patch=train_opt.points_per_patch, sub_sample_size=train_opt.sub_sample_size,
                          net_size=getattr(train_opt, 'net_size', 1024), device=dev_index,
                          precision=getattr(eval_opt, 'precision', 'tc'), guard_band=getattr(eval_opt, 'guard_band', 0.05),
-                         output_dim=_output_dim(train_opt))
+                         output_dim=_output_dim(train_opt), single_transformer=single)
         uniform = bool(getattr(train_opt, 'uniform_subsample', 0))
         model_out_dir = os.path.join(eval_opt.outdir, 'rec' if eval_opt.reconstruction else 'eval')
         os.makedirs(model_out_dir, exist_ok=True)

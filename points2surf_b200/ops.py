@@ -30,9 +30,11 @@ class Engine:
     """Device-resident model (replaces make_regressor, source/points_to_surf_eval.py:150-171)."""
 
     def __init__(self, state_dict, use_point_stn, shared_transformer, points_per_patch=300,
-                 sub_sample_size=1000, net_size=1024, device=0, precision='fp32', guard_band=0.0, output_dim=2):
+                 sub_sample_size=1000, net_size=1024, device=0, precision='fp32', guard_band=0.0, output_dim=2,
+                 single_transformer=False):
         """output_dim 2: logits (|d| logit, sign logit); output_dim 1: the regression head's signed-distance logit.
-        reconstruct() applies the matching post-process."""
+        reconstruct() applies the matching post-process.  single_transformer: the shared-encoder ablation (one
+        feat_local_global over patch + sub-sample; needs use_point_stn and no shared_transformer)."""
         self.lib = _lib.load()
         if not torch.cuda.is_available():
             raise P2SError('CUDA is not available: points2surf_b200 has no CPU fallback')
@@ -40,13 +42,14 @@ class Engine:
         self.cfg = ModelConfig(int(bool(use_point_stn)), int(bool(shared_transformer)), int(points_per_patch),
                                int(sub_sample_size), int(net_size))
         self.output_dim = int(output_dim)
-        blob = _weights.pack_blob(state_dict, use_point_stn, shared_transformer, self.output_dim)
-        expect = self.lib.p2s_model_blob_floats_ex(C.byref(self.cfg), self.output_dim)
+        self.single_transformer = int(bool(single_transformer))
+        blob = _weights.pack_blob(state_dict, use_point_stn, shared_transformer, self.output_dim, self.single_transformer)
+        expect = self.lib.p2s_model_blob_floats_enc(C.byref(self.cfg), self.output_dim, self.single_transformer)
         if blob.size != expect:
             raise P2SError('state_dict does not match the model config (%d floats, expected %d)' % (blob.size, expect))
         h = C.c_void_p()
-        check(self.lib.p2s_model_create_ex(C.byref(self.cfg), self.output_dim, blob.ctypes.data_as(C.c_void_p), blob.size,
-                                           self.device.index, C.byref(h)))
+        check(self.lib.p2s_model_create_enc(C.byref(self.cfg), self.output_dim, self.single_transformer,
+                                            blob.ctypes.data_as(C.c_void_p), blob.size, self.device.index, C.byref(h)))
         self.handle = h
         self.P, self.S = int(points_per_patch), int(sub_sample_size)
         self.set_precision(precision, guard_band)
@@ -68,7 +71,8 @@ class Engine:
             pass
 
     def forward_with_aux(self, patch_pts_ps, pts_sub_sample_ms, imp_surf_query_point_ms):
-        """-> (logits, dict(trans [B,3,3], feat_local_max [B,1024], feat_global_max [B,1024])) -- parity diagnostics."""
+        """-> (logits, dict(trans [B,3,3], feat_local_max [B,1024], feat_global_max [B,1024])) -- parity diagnostics.
+        A single_transformer engine has one encoder: dict(trans [B,3,3], feat_max [B,1024])."""
         B = patch_pts_ps.shape[0]
         aux = torch.zeros((B, 2064), dtype=torch.float32, device=patch_pts_ps.device)
         check(self.lib.p2s_model_set_debug_aux(self.handle, _ptr(aux)))
@@ -77,6 +81,8 @@ class Engine:
             torch.cuda.synchronize()
         finally:
             check(self.lib.p2s_model_set_debug_aux(self.handle, None))
+        if self.single_transformer:
+            return out, {'trans': aux[:, :9].reshape(B, 3, 3), 'feat_max': aux[:, 9:1033]}
         return out, {'trans': aux[:, :9].reshape(B, 3, 3), 'feat_local_max': aux[:, 9:1033], 'feat_global_max': aux[:, 1033:2057]}
 
     def profile_enable(self, on=True):

@@ -23,6 +23,8 @@ VARIANTS = {
     # experiments/train_p2s_regression.sh: the per-branch QSTN network with the distance-weighted sub-sample and the
     # regression head (outputs imp_surf patch_pts_ids p_index: fc4 128 -> 1)
     'regression': dict(use_point_stn=1, shared_transformer=0, uniform_subsample=0, output_dim=1),
+    # experiments/train_p2s_shared_encoder.sh: one encoder (feat_local_global, its own QSTN) over patch + sub-sample
+    'shared_encoder': dict(use_point_stn=1, shared_transformer=0, uniform_subsample=0, single_transformer=1),
 }
 
 
@@ -35,7 +37,7 @@ def make_train_opt(variant='vanilla', points_per_patch=300, sub_sample_size=1000
         name='p2s_' + variant, net_size=net_size, points_per_patch=points_per_patch,
         sub_sample_size=sub_sample_size, patch_radius=0.0, patch_center='mean',
         use_point_stn=v['use_point_stn'], use_feat_stn=1, sym_op='max',
-        single_transformer=0, shared_transformer=v['shared_transformer'],
+        single_transformer=v.get('single_transformer', 0), shared_transformer=v['shared_transformer'],
         uniform_subsample=v['uniform_subsample'], fixed_subsample=0,
         outputs=(['imp_surf'] if v.get('output_dim', 2) == 1 else ['imp_surf_magnitude', 'imp_surf_sign']) +
                 ['patch_pts_ids', 'p_index'],
@@ -45,7 +47,8 @@ def make_train_opt(variant='vanilla', points_per_patch=300, sub_sample_size=1000
 def _layer_specs(variant, net=1024):
     from .arch import layer_specs
     v = VARIANTS[variant]
-    return layer_specs(v['use_point_stn'], v['shared_transformer'], net, v.get('output_dim', 2))
+    return layer_specs(v['use_point_stn'], v['shared_transformer'], net, v.get('output_dim', 2),
+                       bool(v.get('single_transformer', 0)))
 
 
 def make_state_dict_numpy(variant='vanilla', seed=0, net=1024, module_prefix=''):
@@ -76,19 +79,24 @@ FITTED_FC4 = os.path.join(os.path.dirname(os.path.abspath(__file__)), 'fitted_fc
 # the regression head's fitted fc4 [1,128] (tests/golden/make_regression_golden.py fit), as text: every value is written
 # with enough digits to give back the same float32
 FITTED_FC4_REGRESSION = os.path.join(os.path.dirname(os.path.abspath(__file__)), 'fitted_fc4_regression.json')
+# the shared encoder's fitted fc4 [2,128] (tests/golden/make_shared_encoder_golden.py fit), as text like the regression head
+FITTED_FC4_SHARED_ENCODER = os.path.join(os.path.dirname(os.path.abspath(__file__)), 'fitted_fc4_shared_encoder.json')
+_FITTED_FC4_JSON = {'regression': FITTED_FC4_REGRESSION, 'shared_encoder': FITTED_FC4_SHARED_ENCODER}
 
 
 def fitted_fc4(variant, seed):
     """Last layer (fc4 weight [output_dim,128], bias [output_dim]) fitted on a 10k-point sphere so that the otherwise
     rand-init checkpoint `make_state_dict(variant, seed)` produces a surface-like SDF (tests/golden/make_e2e_golden.py
-    and, for 'regression', tests/golden/make_regression_golden.py: ridge regression on the fc3 activations against the
-    analytic signed distance; everything in front of fc4 stays random).
+    and, for 'regression' and 'shared_encoder', tests/golden/make_regression_golden.py and
+    tests/golden/make_shared_encoder_golden.py: ridge regression on the fc3 activations against the analytic signed
+    distance; everything in front of fc4 stays random).
     Only the (variant, seed) pairs the files were fitted for are available."""
-    if variant == 'regression':
-        with open(FITTED_FC4_REGRESSION) as fp:
+    if variant in _FITTED_FC4_JSON:
+        path = _FITTED_FC4_JSON[variant]
+        with open(path) as fp:
             f = json.load(fp)
         if int(f['seed']) != int(seed):
-            raise ValueError('no fitted fc4 for (%s, seed %d) in %s' % (variant, seed, FITTED_FC4_REGRESSION))
+            raise ValueError('no fitted fc4 for (%s, seed %d) in %s' % (variant, seed, path))
         return np.array(f['weight'], np.float32), np.array(f['bias'], np.float32)
     f = np.load(FITTED_FC4)
     if variant + '_seed' not in f or int(f[variant + '_seed']) != int(seed):

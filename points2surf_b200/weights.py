@@ -48,8 +48,10 @@ def _feat(sd, p, qstn):
     return out
 
 
-def pack_blob(state_dict, use_point_stn, shared_transformer, output_dim=2):
-    """output_dim: 2 for the (imp_surf_magnitude, imp_surf_sign) head, 1 for the regression head (imp_surf)."""
+def pack_blob(state_dict, use_point_stn, shared_transformer, output_dim=2, single_transformer=False):
+    """output_dim: 2 for the (imp_surf_magnitude, imp_surf_sign) head, 1 for the regression head (imp_surf).
+    single_transformer: the shared-encoder ablation (one `feat_local_global` with its own QSTN, `fc1_local_global`
+    1024 -> 1024); it needs use_point_stn and no shared_transformer, like the published checkpoints."""
     sd = strip_module_prefix(state_dict)
     if output_dim not in (1, 2):
         raise ValueError('Unsupported output_dim %r: 1 (imp_surf) or 2 (imp_surf_magnitude, imp_surf_sign)' % (output_dim,))
@@ -57,10 +59,16 @@ def pack_blob(state_dict, use_point_stn, shared_transformer, output_dim=2):
     if fc4[0] != output_dim:
         raise ValueError('fc4 has %d outputs, expected output_dim %d' % (fc4[0], output_dim))
     parts = []
-    if use_point_stn and shared_transformer:
-        parts += _stn(sd, 'point_stn.')
-    parts += _feat(sd, 'feat_local.', False)
-    parts += _feat(sd, 'feat_global.', bool(use_point_stn and not shared_transformer))
-    parts += fold(sd, 'fc1_local', 'bn1_local') + fold(sd, 'fc1_global', 'bn1_global')
+    if single_transformer:
+        if not use_point_stn or shared_transformer:
+            raise ValueError('Unsupported option: single_transformer=1 needs use_point_stn=1 and shared_transformer=0')
+        parts += _feat(sd, 'feat_local_global.', True)
+        parts += fold(sd, 'fc1_local_global', 'bn1_local_global')
+    else:
+        if use_point_stn and shared_transformer:
+            parts += _stn(sd, 'point_stn.')
+        parts += _feat(sd, 'feat_local.', False)
+        parts += _feat(sd, 'feat_global.', bool(use_point_stn and not shared_transformer))
+        parts += fold(sd, 'fc1_local', 'bn1_local') + fold(sd, 'fc1_global', 'bn1_global')
     parts += fold(sd, 'fc2', 'bn2') + fold(sd, 'fc3', 'bn3') + fold(sd, 'fc4', None)
     return np.ascontiguousarray(np.concatenate(parts), dtype=np.float32)
