@@ -477,12 +477,17 @@ int p2s_op_gemm_tn(const float* A, int64_t a_stride_z, int lda, const float* B, 
                    void* stream);
 /* out[z][c][r] = in[z][r][c] */
 int p2s_op_transpose(const float* in, float* out, int rows, int cols, int batch, void* stream);
-/* BatchNorm1d(train): s1 = sum x, s2 = sum x^2 over the M rows (f64 [C] each) */
+/* s1 = sum x, s2 = sum x^2 over the M rows (f64 [C] each) */
 int p2s_op_col_stats(const float* x, int64_t M, int C, double* s1, double* s2, void* stream);
 int p2s_op_col_sum(const float* x, int64_t M, int C, double* s1, void* stream);
-/* mean, invstd = 1/sqrt(biased var + eps); running stats updated like torch (unbiased var) when non-NULL */
+/* mean, invstd = 1/sqrt(biased var + eps) from the sums of p2s_op_col_stats; running stats updated like torch (unbiased
+ * var) when non-NULL.  var = s2/M - (s1/M)^2 cancels once |mean| >> std: BatchNorm uses p2s_op_bn_stats. */
 int p2s_op_bn_finalize(const double* s1, const double* s2, int64_t M, int C, float eps, float momentum,
                        float* mean, float* invstd, float* running_mean, float* running_var, void* stream);
+/* BatchNorm1d(train) statistics of x [M, C]: mean, invstd and the running stats as p2s_op_bn_finalize, from f64 sums
+ * of x - x[0] and (x - x[0])^2 (left in s1, s2, f64 [C] each), so invstd is accurate to ~2^-24 for any |mean| / std */
+int p2s_op_bn_stats(const float* x, int64_t M, int C, float eps, float momentum, double* s1, double* s2,
+                    float* mean, float* invstd, float* running_mean, float* running_var, void* stream);
 /* y = act(gamma (z - mean) invstd + beta) */
 int p2s_op_bn_apply(const float* z, int64_t M, int C, const float* mean, const float* invstd,
                     const float* gamma, const float* beta, int relu, float* y, void* stream);

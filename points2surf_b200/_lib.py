@@ -96,6 +96,7 @@ SIGNATURES = {
     'p2s_op_col_stats': (C.c_int, [_vp, _i64, _i32, _vp, _vp, _vp]),
     'p2s_op_col_sum': (C.c_int, [_vp, _i64, _i32, _vp, _vp]),
     'p2s_op_bn_finalize': (C.c_int, [_vp, _vp, _i64, _i32, _f32, _f32, _vp, _vp, _vp, _vp, _vp]),
+    'p2s_op_bn_stats': (C.c_int, [_vp, _i64, _i32, _f32, _f32, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     'p2s_op_bn_apply': (C.c_int, [_vp, _i64, _i32, _vp, _vp, _vp, _vp, _i32, _vp, _vp]),
     'p2s_op_bn_backward': (C.c_int, [_vp, _vp, _vp, _i64, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     'p2s_op_bn_maxpool_fwd': (C.c_int, [_vp, _i64, _i32, _i32, _vp, _vp, _vp, _vp, _i32, _vp, _vp, _vp]),

@@ -603,6 +603,10 @@ P2S_OP(p2s_op_bn_finalize, (const double* s1, const double* s2, int64_t M, int C
                             float* invstd, float* running_mean, float* running_var, void* stream),
        P2S_CHECK(s1 && s2 && mean && invstd && M > 0, "bad argument");
         op_bn_finalize(s1, s2, M, C, eps, momentum, mean, invstd, running_mean, running_var, as_stream(stream)))
+P2S_OP(p2s_op_bn_stats, (const float* x, int64_t M, int C, float eps, float momentum, double* s1, double* s2, float* mean,
+                         float* invstd, float* running_mean, float* running_var, void* stream),
+       P2S_CHECK(x && s1 && s2 && mean && invstd && M > 0, "bad argument");
+        op_bn_stats(x, M, C, eps, momentum, s1, s2, mean, invstd, running_mean, running_var, as_stream(stream)))
 P2S_OP(p2s_op_bn_apply, (const float* z, int64_t M, int C, const float* mean, const float* invstd, const float* gamma,
                          const float* beta, int relu, float* y, void* stream),
        P2S_CHECK(z && mean && invstd && gamma && beta && y, "null argument");

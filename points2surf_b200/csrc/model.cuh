@@ -154,6 +154,8 @@ void op_col_stats(const float* x, int64_t M, int C, double* s1, double* s2, cuda
 void op_col_sum(const float* x, int64_t M, int C, double* s1, cudaStream_t st);
 void op_bn_finalize(const double* s1, const double* s2, int64_t M, int C, float eps, float momentum, float* mean,
                     float* invstd, float* running_mean, float* running_var, cudaStream_t st);
+void op_bn_stats(const float* x, int64_t M, int C, float eps, float momentum, double* s1, double* s2, float* mean,
+                 float* invstd, float* running_mean, float* running_var, cudaStream_t st);
 void op_bn_apply(const float* z, int64_t M, int C, const float* mean, const float* invstd, const float* gamma,
                  const float* beta, bool relu, float* y, cudaStream_t st);
 void op_bn_backward(const float* dy, const float* z, const float* y_or_null, int64_t M, int C, const float* mean,

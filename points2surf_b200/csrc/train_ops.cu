@@ -6,7 +6,8 @@
 //   forward  Z = X W^T            -> launch_gemm_nt (net_fp32.cu)
 //   dX = dZ W = dZ (W^T)^T        -> launch_gemm_nt on the transposed weight (transpose_kernel)
 //   dW = dZ^T X                   -> gemm_tn_kernel below (contraction over the rows, split over CTAs, atomics)
-// Column reductions (BatchNorm statistics, bias / gamma / beta gradients) accumulate in f64.
+// Column reductions (BatchNorm statistics, bias / gamma / beta gradients) accumulate in f64 from the first term, and the
+// BatchNorm statistics are sums of x - x[0] so the variance's error does not grow with the column's mean.
 #include "model.cuh"
 
 namespace p2s {
@@ -92,9 +93,12 @@ __global__ void transpose_kernel(const float* __restrict__ in, float* __restrict
 }
 
 // ---------------------------------------------------------------- column reductions over [M, C] (f64 accumulators)
-// MODE 0: s1 += sum x, s2 += sum x*x                      (BatchNorm statistics)
+// MODE 0: s1 += sum d, s2 += sum d*d, d = x - x0[c]          (BatchNorm statistics; x0 = z, the shift row, or none)
 // MODE 1: s1 += sum g, s2 += sum g * xhat, g = dy * (y > 0 if y), xhat = (z - mean) * invstd   (BatchNorm backward)
 // MODE 2: s1 += sum x                                      (bias gradient)
+// Every sum is f64 from the first term: each product of two fp32 values is exact in f64, so the only roundings are the
+// f64 additions.  The shift makes the variance's cancellation s2/M - (s1/M)^2 independent of the column's mean: with
+// d = x - x0 exact in f64 it is relative to 1 + ((mean - x0) / std)^2 instead of 1 + (mean / std)^2.
 template <int MODE>
 __global__ void __launch_bounds__(256)
 col_reduce_kernel(const float* __restrict__ x, const float* __restrict__ z, const float* __restrict__ y,
@@ -102,44 +106,49 @@ col_reduce_kernel(const float* __restrict__ x, const float* __restrict__ z, cons
                   int64_t rows_per_block, double* __restrict__ s1, double* __restrict__ s2) {
     const int c = blockIdx.x * 32 + threadIdx.x;
     const int64_t r_begin = (int64_t)blockIdx.y * rows_per_block, r_end = min(M, r_begin + rows_per_block);
-    float a1 = 0.f, a2 = 0.f;
+    double a1 = 0.0, a2 = 0.0;
     if (c < C) {
         float mu = 0.f, is = 0.f;
+        double x0 = 0.0;
         if (MODE == 1) { mu = mean[c]; is = invstd[c]; }
+        if (MODE == 0 && z) x0 = (double)z[c];   // z: the shift row in MODE 0
 #pragma unroll 4
         for (int64_t r = r_begin + threadIdx.y; r < r_end; r += 8) {
             const int64_t e = r * C + c;
             float v = x[e];
-            if (MODE == 0) { a1 += v; a2 = fmaf(v, v, a2); }
+            if (MODE == 0) { const double d = (double)v - x0; a1 += d; a2 = fma(d, d, a2); }
             else if (MODE == 1) {
                 if (y && !(y[e] > 0.f)) v = 0.f;
-                a1 += v;
-                a2 = fmaf(v, (z[e] - mu) * is, a2);
-            } else a1 += v;
+                a1 += (double)v;
+                a2 = fma((double)v, (double)((z[e] - mu) * is), a2);
+            } else a1 += (double)v;
         }
     }
-    __shared__ float r1[8][32], r2[8][32];
+    __shared__ double r1[8][32], r2[8][32];
     r1[threadIdx.y][threadIdx.x] = a1;
     r2[threadIdx.y][threadIdx.x] = a2;
     __syncthreads();
     if (threadIdx.y == 0 && c < C) {
         double d1 = 0.0, d2 = 0.0;
 #pragma unroll
-        for (int j = 0; j < 8; ++j) { d1 += (double)r1[j][threadIdx.x]; d2 += (double)r2[j][threadIdx.x]; }
+        for (int j = 0; j < 8; ++j) { d1 += r1[j][threadIdx.x]; d2 += r2[j][threadIdx.x]; }
         atomicAdd(s1 + c, d1);
         if (MODE != 2) atomicAdd(s2 + c, d2);
     }
 }
 
-// mean / invstd from the sums; running statistics like torch.nn.BatchNorm1d (momentum 0.1, unbiased running var)
-__global__ void bn_finalize_kernel(const double* __restrict__ s1, const double* __restrict__ s2, int64_t M, int C,
-                                   float eps, float momentum, float* __restrict__ mean, float* __restrict__ invstd,
+// mean / invstd from the sums of col_reduce_kernel<0> about the shift row x0 (NULL: unshifted sums); running statistics
+// like torch.nn.BatchNorm1d (momentum 0.1, unbiased running var)
+__global__ void bn_finalize_kernel(const double* __restrict__ s1, const double* __restrict__ s2,
+                                   const float* __restrict__ x0, int64_t M, int C, float eps, float momentum,
+                                   float* __restrict__ mean, float* __restrict__ invstd,
                                    float* __restrict__ running_mean, float* __restrict__ running_var) {
     int c = blockIdx.x * blockDim.x + threadIdx.x;
     if (c >= C) return;
-    double mu = s1[c] / (double)M;
-    double var = s2[c] / (double)M - mu * mu;
+    const double md = s1[c] / (double)M;   // mean - x0
+    double var = s2[c] / (double)M - md * md;
     if (var < 0.0) var = 0.0;
+    const double mu = (x0 ? (double)x0[c] : 0.0) + md;
     mean[c] = (float)mu;
     invstd[c] = (float)(1.0 / sqrt(var + (double)eps));
     if (running_mean) running_mean[c] = (1.f - momentum) * running_mean[c] + momentum * (float)mu;
@@ -205,7 +214,8 @@ __global__ void bn_maxpool_fwd_kernel(const float* __restrict__ z, int64_t B, in
     for (int i = 0; i < npts; ++i) {
         float v = fmaf(a, p[(int64_t)i * C] - mu, bt);
         if (relu) v = fmaxf(v, 0.f);
-        if (v > best || i == 0) { best = v; bi = i; }   // first maximum, like torch.max / MaxPool1d
+        // first maximum, like torch.max / MaxPool1d; the first NaN wins and stays, like maxpool_fwd_kernel
+        if (v > best || i == 0 || (v != v && !(best != best))) { best = v; bi = i; }
     }
     out[b * C + c] = best;
     arg[b * C + c] = bi;
@@ -219,25 +229,25 @@ bn_maxpool_bwd_reduce_kernel(const float* __restrict__ dout, const int32_t* __re
                              int C, int relu, int64_t rows_per_block, double* __restrict__ s1, double* __restrict__ s2) {
     const int c = blockIdx.x * 32 + threadIdx.x;
     const int64_t b0 = (int64_t)blockIdx.y * rows_per_block, b1 = min(B, b0 + rows_per_block);
-    float a1 = 0.f, a2 = 0.f;
+    double a1 = 0.0, a2 = 0.0;   // f64 from the first term, like col_reduce_kernel<1>
     if (c < C) {
         const float mu = mean[c], is = invstd[c];
         for (int64_t b = b0 + threadIdx.y; b < b1; b += 8) {
             float g = dout[b * C + c];
             if (relu && !(out[b * C + c] > 0.f)) g = 0.f;
             const float xhat = (z[(b * npts + arg[b * C + c]) * (int64_t)C + c] - mu) * is;
-            a1 += g;
-            a2 = fmaf(g, xhat, a2);
+            a1 += (double)g;
+            a2 = fma((double)g, (double)xhat, a2);
         }
     }
-    __shared__ float r1[8][32], r2[8][32];
+    __shared__ double r1[8][32], r2[8][32];
     r1[threadIdx.y][threadIdx.x] = a1;
     r2[threadIdx.y][threadIdx.x] = a2;
     __syncthreads();
     if (threadIdx.y == 0 && c < C) {
         double d1 = 0.0, d2 = 0.0;
 #pragma unroll
-        for (int j = 0; j < 8; ++j) { d1 += (double)r1[j][threadIdx.x]; d2 += (double)r2[j][threadIdx.x]; }
+        for (int j = 0; j < 8; ++j) { d1 += r1[j][threadIdx.x]; d2 += r2[j][threadIdx.x]; }
         atomicAdd(s1 + c, d1);
         atomicAdd(s2 + c, d2);
     }
@@ -489,14 +499,18 @@ static void rowwise_grid(int64_t M, int C, dim3& blk, dim3& g, int64_t& rows_per
     g = dim3((unsigned)cx, (unsigned)cdiv(M, rows_per_block));
 }
 
-// s1, s2: f64 [C], zeroed here
-void op_col_stats(const float* x, int64_t M, int C, double* s1, double* s2, cudaStream_t st) {
+// s1 = sum (x - shift), s2 = sum (x - shift)^2: f64 [C], zeroed here; shift = a row of C values or NULL (no shift)
+static void col_stats(const float* x, const float* shift, int64_t M, int C, double* s1, double* s2, cudaStream_t st) {
     P2S_CUDA(cudaMemsetAsync(s1, 0, sizeof(double) * C, st));
     P2S_CUDA(cudaMemsetAsync(s2, 0, sizeof(double) * C, st));
     if (M <= 0) return;
     dim3 g; int64_t rpb;
     col_reduce_grid(M, C, g, rpb);
-    P2S_LAUNCH(col_reduce_kernel<0>, g, dim3(32, 8), 0, st, x, nullptr, nullptr, nullptr, nullptr, M, C, rpb, s1, s2);
+    P2S_LAUNCH(col_reduce_kernel<0>, g, dim3(32, 8), 0, st, x, shift, nullptr, nullptr, nullptr, M, C, rpb, s1, s2);
+}
+
+void op_col_stats(const float* x, int64_t M, int C, double* s1, double* s2, cudaStream_t st) {
+    col_stats(x, nullptr, M, C, s1, s2, st);
 }
 
 void op_col_sum(const float* x, int64_t M, int C, double* s1, cudaStream_t st) {
@@ -509,7 +523,16 @@ void op_col_sum(const float* x, int64_t M, int C, double* s1, cudaStream_t st) {
 
 void op_bn_finalize(const double* s1, const double* s2, int64_t M, int C, float eps, float momentum, float* mean,
                     float* invstd, float* running_mean, float* running_var, cudaStream_t st) {
-    P2S_LAUNCH(bn_finalize_kernel, (unsigned)cdiv(C, 128), 128, 0, st, s1, s2, M, C, eps, momentum, mean, invstd,
+    P2S_LAUNCH(bn_finalize_kernel, (unsigned)cdiv(C, 128), 128, 0, st, s1, s2, (const float*)nullptr, M, C, eps, momentum,
+               mean, invstd, running_mean, running_var);
+}
+
+// train-mode BatchNorm statistics: the sums are taken about row 0 of x, so the variance's cancellation is relative to
+// the spread of each column about its first value rather than to its mean (col_reduce_kernel); s1, s2 f64 [C] scratch
+void op_bn_stats(const float* x, int64_t M, int C, float eps, float momentum, double* s1, double* s2, float* mean,
+                 float* invstd, float* running_mean, float* running_var, cudaStream_t st) {
+    col_stats(x, x, M, C, s1, s2, st);
+    P2S_LAUNCH(bn_finalize_kernel, (unsigned)cdiv(C, 128), 128, 0, st, s1, s2, x, M, C, eps, momentum, mean, invstd,
                running_mean, running_var);
 }
 

@@ -77,8 +77,7 @@ class CudaPrims:
         invstd = torch.empty_like(mean)
         y = torch.empty_like(z)
         with torch.cuda.device(z.device):
-            check(self.lib.p2s_op_col_stats(_ptr(z), M, Cc, _ptr(s[0]), _ptr(s[1]), _stream()))
-            check(self.lib.p2s_op_bn_finalize(_ptr(s[0]), _ptr(s[1]), M, Cc, float(eps), float(momentum), _ptr(mean), _ptr(invstd),
+            check(self.lib.p2s_op_bn_stats(_ptr(z), M, Cc, float(eps), float(momentum), _ptr(s[0]), _ptr(s[1]), _ptr(mean), _ptr(invstd),
                                               _ptr(running_mean) if running_mean is not None else None,
                                               _ptr(running_var) if running_var is not None else None, _stream()))
             check(self.lib.p2s_op_bn_apply(_ptr(z), M, Cc, _ptr(mean), _ptr(invstd), _ptr(_f(gamma, 'gamma')), _ptr(_f(beta, 'beta')),
@@ -117,8 +116,7 @@ class CudaPrims:
         out = torch.empty((B, Cc), dtype=torch.float32, device=z.device)
         arg = torch.empty((B, Cc), dtype=torch.int32, device=z.device)
         with torch.cuda.device(z.device):
-            check(self.lib.p2s_op_col_stats(_ptr(z), M, Cc, _ptr(s[0]), _ptr(s[1]), _stream()))
-            check(self.lib.p2s_op_bn_finalize(_ptr(s[0]), _ptr(s[1]), M, Cc, float(eps), float(momentum), _ptr(mean), _ptr(invstd),
+            check(self.lib.p2s_op_bn_stats(_ptr(z), M, Cc, float(eps), float(momentum), _ptr(s[0]), _ptr(s[1]), _ptr(mean), _ptr(invstd),
                                               _ptr(running_mean) if running_mean is not None else None,
                                               _ptr(running_var) if running_var is not None else None, _stream()))
             check(self.lib.p2s_op_bn_maxpool_fwd(_ptr(z), B, npts, Cc, _ptr(mean), _ptr(invstd), _ptr(_f(gamma, 'gamma')),
