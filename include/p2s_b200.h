@@ -359,6 +359,60 @@ typedef struct {
 int p2s_mesh_clean_dev(const float* verts, int64_t V, const int32_t* faces, int64_t F, float* verts_out, int64_t vcap,
                        int32_t* faces_out, int64_t fcap, p2s_clean_report* report_host, void* stream);
 
+/* ------------------------------------------------------------------ mesh repair (hole filling) -- */
+/* The first four filters of the reference's hole_filling_mesh_simp.mlx (dataset_for_deepsdf.py), which it runs through
+ * meshlabserver before computing DeepSDF's far-sample distances.  Meshlab's exact choices are not pinned; these are this
+ * project's rules, in this order:
+ *   1. non-manifold edges, removing faces: every undirected edge with c > 2 faces drops its c - 2 smallest faces by
+ *      float64 squared area |(b - a) x (c - a)|^2 (ties: the higher face index is dropped first).  All edges are judged
+ *      on the input faces at once; a face dropped by any edge is removed.  Afterwards no edge has more than two faces.
+ *   2. non-manifold edges, splitting vertices: a no-op after 1 (no edge has more than two faces), so nothing is done.
+ *   3. non-manifold vertices, splitting (VertDispRatio 0): the faces around a vertex are joined into fans over the edges
+ *      of that vertex that have two faces.  A vertex with k > 1 fans gets k - 1 copies at the same position: the fan
+ *      holding the lowest face index keeps the vertex; the copies are appended after the input vertices in order of
+ *      their fan's lowest face index (ties, one face opening fans at two vertices: its corner order 0, 1, 2).
+ *   4. close holes (MaxHoleSize, SelfIntersection): after 3 every boundary vertex has exactly two boundary edges, so the
+ *      boundary edges form simple loops.  A loop of L <= max_hole_size edges is filled by ear cutting:
+ *      - the walk starts at the loop's lowest vertex v towards the neighbour x whose boundary edge runs x -> v in its
+ *        face (the lower neighbour when both or neither do), and goes on around the loop; every fill face (prev, tip,
+ *        next) follows the walk, so it runs against the boundary edges it closes;
+ *      - the plane: the float64 Newell normal n of the walk; u = n x e_k / |n x e_k| for the axis k of smallest |n_k|
+ *        (the lowest k on ties), w = (n / |n|) x u; vertex i goes to (p_i . u, p_i . w).  A zero n leaves no valid ear;
+ *      - an ear is convex when the 2D cross product of (tip - prev, next - tip) is > 0; convex ears are tried by the
+ *        smallest tip angle first (the largest cos of the 2D angle), ties by the lowest tip vertex id, and the first
+ *        valid one is cut, until the loop is a triangle, which is cut the same way;
+ *      - while more than three loop vertices remain, an ear is not valid when its new edge (next, prev) is already an
+ *        edge of the mesh (it would get a third face);
+ *      - an ear is not valid when another remaining loop vertex lies inside or on its 2D triangle (it would overlap the
+ *        faces beyond the loop's boundary: the planar form of the intersection test), or, with prevent_self_intersection,
+ *        when an edge of the ear crosses the interior of a face incident to a loop vertex or of a triangle already
+ *        added to this loop, or an edge of such a face crosses the ear's interior.  A crossing is strict: the segment's
+ *        ends lie strictly on both sides of the triangle's plane and it passes strictly inside all three edges, each side
+ *        a float64 signed volume ((b-a) x (c-a)) . (d-a), taken as 0 when two of its four points coincide.  Coplanar
+ *        contact and touching at shared vertices or edges is not a crossing;
+ *      - when no convex ear is valid, the faces cut so far are dropped and the loop stays open (counted in
+ *        holes_left_open, like the loops longer than max_hole_size).  Triangles added to other loops are not tested.
+ *   Decimation to 100 000 faces (the .mlx's last filter) is not done: the repaired mesh is only a signed-distance target.
+ * Output order: vertices = the input vertices, then the copies of 3; faces = the faces kept by 1 in input order (with the
+ * indices of 3), then the fill faces, loop by loop in order of each loop's lowest vertex id, in cutting order.
+ *   verts [V,3] fp32, faces [F,3] int32: every index in [0, V) and three distinct indices per face, else an error.
+ *   max_hole_size in [0, 128] (30 in the .mlx); prevent_self_intersection 0/1 (1 in the .mlx).
+ *   verts_out [vcap,3] fp32, faces_out [fcap,3] int32: vcap >= V + 3 F and fcap >= 4 F always suffice; a capacity that
+ *   turns out too small is an error, not a truncation.
+ * Bitwise deterministic (integer atomics only, float64 geometry in a fixed order).  sync: several read-backs. */
+typedef struct {
+    int64_t vertices_in, faces_in, vertices_out, faces_out;
+    int64_t faces_removed;       /* by rule 1 */
+    int64_t vertices_split;      /* copies appended by rule 3 */
+    int64_t holes_closed;        /* loops filled by rule 4 */
+    int64_t holes_left_open;     /* loops longer than max_hole_size, and loops without a valid ear */
+    int64_t faces_added;
+} p2s_repair_stats;
+
+int p2s_mesh_repair_dev(const float* verts, int64_t V, const int32_t* faces, int64_t F, int32_t max_hole_size,
+                        int32_t prevent_self_intersection, float* verts_out, int64_t vcap, int32_t* faces_out, int64_t fcap,
+                        p2s_repair_stats* stats_host, void* stream);
+
 /* ------------------------------------------------------------------ screened Poisson baseline --- */
 /* Screened Poisson surface reconstruction from oriented points, the SPSR baseline of eval_dataset.py:142-158 (which
  * the reference runs through meshlabserver with poisson.mlx).  The discrete system:

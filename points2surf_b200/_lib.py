@@ -34,6 +34,12 @@ class CleanReport(C.Structure):
         [('volume', C.c_double)]
 
 
+class RepairStats(C.Structure):
+    _fields_ = [(n, C.c_int64) for n in (
+        'vertices_in', 'faces_in', 'vertices_out', 'faces_out', 'faces_removed', 'vertices_split', 'holes_closed',
+        'holes_left_open', 'faces_added')]
+
+
 class PoissonConfig(C.Structure):
     _fields_ = [('depth', C.c_int32), ('point_weight', C.c_float), ('scale', C.c_float), ('iters', C.c_int32)]
 
@@ -117,6 +123,8 @@ SIGNATURES = {
     'p2s_range_scan_dev': (C.c_int, [_vp, _i64, _vp, _i64, _vp, _i64, C.POINTER(ScanConfig), C.c_uint64, _vp, _vp, _vp,
                                      _i64, _vp, C.POINTER(_i64), _vp]),
     'p2s_mesh_clean_dev': (C.c_int, [_vp, _i64, _vp, _i64, _vp, _i64, _vp, _i64, C.POINTER(CleanReport), _vp]),
+    'p2s_mesh_repair_dev': (C.c_int, [_vp, _i64, _vp, _i64, _i32, _i32, _vp, _i64, _vp, _i64, C.POINTER(RepairStats),
+                                      _vp]),
     'p2s_poisson_solve_dev': (C.c_int, [_vp, _vp, _i64, C.POINTER(PoissonConfig), _vp, _i64, C.POINTER(PoissonReport),
                                         _vp]),
     'p2s_point_normals_dev': (C.c_int, [_vp, _i64, _i32, _i32, C.POINTER(C.c_double), _vp, _vp, C.POINTER(NormalsStats),

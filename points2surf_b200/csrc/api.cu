@@ -552,6 +552,16 @@ int p2s_mesh_clean_dev(const float* verts, int64_t V, const int32_t* faces, int6
     });
 }
 
+int p2s_mesh_repair_dev(const float* verts, int64_t V, const int32_t* faces, int64_t F, int32_t max_hole_size,
+                        int32_t prevent_self_intersection, float* verts_out, int64_t vcap, int32_t* faces_out, int64_t fcap,
+                        p2s_repair_stats* stats_host, void* stream) {
+    return guarded([&] {
+        P2S_CHECK((verts || V == 0) && (faces || F == 0) && stats_host, "null argument");
+        mesh_repair(verts, V, faces, F, max_hole_size, prevent_self_intersection != 0, verts_out, vcap, faces_out, fcap,
+                    stats_host, as_stream(stream));
+    });
+}
+
 int p2s_poisson_solve_dev(const float* pts, const float* normals, int64_t N, const p2s_poisson_config* cfg, float* values,
                           int64_t vcap, p2s_poisson_report* report_host, void* stream) {
     return guarded([&] {

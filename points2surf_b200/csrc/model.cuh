@@ -134,6 +134,10 @@ void range_scan(const float* verts, int64_t V, const int32_t* faces, int64_t F, 
 // meshclean.cu
 void mesh_clean(const float* verts, int64_t V, const int32_t* faces, int64_t F, float* verts_out, int64_t vcap,
                 int32_t* faces_out, int64_t fcap, p2s_clean_report* report, cudaStream_t st);
+// meshrepair.cu
+void mesh_repair(const float* verts, int64_t V, const int32_t* faces, int64_t F, int max_hole_size,
+                 bool prevent_self_intersection, float* verts_out, int64_t vcap, int32_t* faces_out, int64_t fcap,
+                 p2s_repair_stats* stats, cudaStream_t st);
 // poisson.cu
 void poisson_solve(const float* pts, const float* normals, int64_t N, const p2s_poisson_config& cfg, float* values,
                    int64_t cap, p2s_poisson_report* report, cudaStream_t st);

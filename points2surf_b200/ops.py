@@ -367,6 +367,28 @@ def mesh_clean(verts, faces):
     return vout[:rep.vertices_out], fout[:rep.faces_out], report
 
 
+def mesh_repair(verts, faces, max_hole_size=30, prevent_self_intersection=True):
+    """The first four filters of the reference's hole_filling_mesh_simp.mlx (rules and output order in
+    include/p2s_b200.h): drop the smallest faces of non-manifold edges, split non-manifold vertices, close boundary loops
+    of at most `max_hole_size` edges by ear cutting, without self-intersections when `prevent_self_intersection`.
+    -> (verts [V',3] fp32, faces [F',3] int32, stats dict of p2s_repair_stats)."""
+    verts = _dev(verts, torch.float32, 'verts')
+    faces = _dev(faces, torch.int32, 'faces')
+    if verts.dim() != 2 or verts.shape[1] != 3 or faces.dim() != 2 or faces.shape[1] != 3:
+        raise P2SError('verts and faces must have shape [n, 3]')
+    V, F = verts.shape[0], faces.shape[0]
+    vcap, fcap = V + 3 * F, 4 * F
+    vout = torch.empty((max(vcap, 1), 3), dtype=torch.float32, device=verts.device)
+    fout = torch.empty((max(fcap, 1), 3), dtype=torch.int32, device=verts.device)
+    st = _lib.RepairStats()
+    with torch.cuda.device(verts.device):
+        check(_lib.load().p2s_mesh_repair_dev(_ptr(verts), V, _ptr(faces), F, int(max_hole_size),
+                                              int(bool(prevent_self_intersection)), _ptr(vout), vcap, _ptr(fout), fcap,
+                                              C.byref(st), _stream()))
+    stats = {name: getattr(st, name) for name, _ in _lib.RepairStats._fields_}
+    return vout[:st.vertices_out], fout[:st.faces_out], stats
+
+
 def poisson_solve(pts, normals, depth=8, point_weight=4.0, scale=1.1, iters=8):
     """Screened Poisson solve on the dense (2^depth + 1)^3 node grid (system, solver and deviations from PoissonRecon in
     include/p2s_b200.h).  pts, normals [N,3] fp32; zero normals drop their point.
