@@ -429,7 +429,8 @@ int p2s_mesh_repair_dev(const float* verts, int64_t V, const int32_t* faces, int
  *   solve   (L + S) chi = b by conjugate gradients preconditioned with one symmetric multigrid V-cycle over depths
  *           depth..2 (exact Galerkin levels, `iters` damped-Jacobi sweeps before and after each coarse correction, 128
  *           sweeps on depth 2); stop at ||b - A chi|| / ||b|| <= 1e-5, after 100 iterations, or when the residual has
- *           not reached a new minimum for 10 iterations
+ *           not reached a new minimum for 10 iterations.  point_weight 0 makes S = 0 and the system singular (L 1 = 0,
+ *           1^T b = 0): chi is then the solution of mean zero over the nodes
  *   iso     sum a_p chi(p) / sum a_p
  * values [(2^depth+1)^3] fp32 = iso - chi at node (i, j, k), index (i R + j) R + k with R = 2^depth + 1: positive inside,
  * zero on the surface, so p2s_marching_cubes_dev(values, R, 0) extracts it; node (i, j, k) is at world position

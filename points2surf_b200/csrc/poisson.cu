@@ -13,7 +13,8 @@
 //   6. conjugate gradients preconditioned by one symmetric V-cycle: `iters` damped-Jacobi sweeps before and after the
 //      coarse correction on every level (D = diag L + row sums of S), kCoarseSweeps sweeps on the 5^3 nodes of depth 2;
 //      L is the matrix-free 27-point Q1 stencil, restriction P^T and prolongation P gather from the nested grid
-//   7. iso = sum a_p chi(p) / sum a_p; the output is iso - chi (positive inside) in fp32
+//   7. point_weight 0 (singular): chi -= mean(chi).  iso = sum a_p chi(p) / sum a_p; the output is iso - chi (positive
+//      inside) in fp32
 // No float atomics: every sum runs in a fixed order, so the output is bitwise identical across runs.
 #include "common.cuh"
 #include <algorithm>
@@ -37,7 +38,7 @@ constexpr int kMaxIters = 100;        // ... or after kMaxIters iterations ...
 constexpr int kStallIters = 10;       // ... or when the residual has not reached a new minimum for kStallIters
 
 enum { OP_APPLY, OP_RESIDUAL, OP_JACOBI };
-enum { SC_RZ0, SC_RZ1, SC_PQ, SC_RR, SC_AREA, SC_ACHI, SC_COUNT };
+enum { SC_RZ0, SC_RZ1, SC_PQ, SC_RR, SC_AREA, SC_ACHI, SC_XSUM, SC_COUNT };
 
 // ---- Morton keys, 9 bits per axis: x in bit 3k+2, y in 3k+1, z in 3k; the parent cell's key is key >> 3
 __host__ __device__ __forceinline__ uint32_t spread3(uint32_t v) {
@@ -283,6 +284,13 @@ poisson_cg_p_kernel(const double* __restrict__ sc, int rz_old, int rz_new, const
     if (v >= nn) return;
     const double beta = sc[rz_old] > 0.0 ? sc[rz_new] / sc[rz_old] : 0.0;
     p[v] = z[v] + beta * p[v];
+}
+
+// x -= mean(x), the sum in sc[SC_XSUM]
+__global__ void __launch_bounds__(256)
+poisson_sub_mean_kernel(const double* __restrict__ sc, double* __restrict__ x, int64_t nn) {
+    const int64_t v = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (v < nn) x[v] -= sc[SC_XSUM] / (double)nn;
 }
 
 // ---- points
@@ -811,6 +819,12 @@ void poisson_solve(const float* pts, const float* nrm, int64_t N, const p2s_pois
         sv.level_op<OP_RESIDUAL>(Fl, X, B, Rr);   // report the true residual, not the recursive one
         sv.dot(Rr, Rr, nn, SC_RR);
         residual = std::sqrt(read_back(sv.sc + SC_RR, 1, st)[0] / bb);
+    }
+    // point_weight 0: S = 0 and L 1 = 0, so chi is only defined up to a constant, which CG leaves wherever the V-cycles
+    // put it; take the solution of mean zero so that chi and iso are defined (values = iso - chi does not change)
+    if (alpha == 0.0) {
+        sv.dot(X, nullptr, nn, SC_XSUM);
+        P2S_LAUNCH(poisson_sub_mean_kernel, grid1d(nn, 256), 256, 0, st, sv.sc, X, nn);
     }
     rep->iterations = it;
     rep->residual = residual;
