@@ -20,6 +20,10 @@
 // Each warpgroup of the CTA streams its own queries (qi = wg, wg + 2, ...) through all layers; the two warpgroups
 // interleave on the SM, so one's FMA / epilogue work overlaps the other's tensor-core work.
 //
+// The fp16 variant runs CTA 2j and 2j+1 as a cluster of two and computes each tile's first and mid layers once: of
+// every pair of tiles (2k, 2k + 1), each CTA produces one, stores its big-layer A fragments into the peer's receive
+// slot (distributed shared memory), runs its own big layer on them, then runs its big layer on the tile the peer sent.
+//
 // The small per-query FC tails between the passes run on the split-precision FC kernel (fc_tc.cu).
 #include "model.cuh"
 #include "tc_ptx.cuh"
@@ -52,7 +56,12 @@ struct Cfg {
     static constexpr uint32_t kWgBytes = kWgWq + 192 * 4;
     static constexpr uint32_t kOffWg = kOffMid + kMidBytes;
     static constexpr uint32_t kOffBias = kOffWg + kWG * kWgBytes;     // [256] mid biases back to back, [64] first-layer bias
-    static constexpr uint32_t kSmemBytes = kOffBias + 320 * 4;
+    // CTA pair exchange (fp16 variant only): per warpgroup one receive slot for the peer's big-layer A fragments and two
+    // mbarriers, full (the peer wrote the slot) and empty (the peer read the slot this CTA wrote into it)
+    static constexpr uint32_t kSlotBytes = PRECISE ? 0u : 8u * 128u * 16u;
+    static constexpr uint32_t kOffSlot = kOffBias + 320 * 4;
+    static constexpr uint32_t kOffXBar = kOffSlot + kWG * kSlotBytes;   // [wg][full, empty]
+    static constexpr uint32_t kSmemBytes = kOffXBar + (PRECISE ? 0u : kWG * 16u);
 };
 static_assert(Cfg<false>::kSmemBytes <= 232448 && Cfg<true>::kSmemBytes <= 232448, "shared memory budget");
 static_assert(Cfg<false>::kRedBytes <= Cfg<false>::kPerqBytes && Cfg<true>::kRedBytes <= Cfg<true>::kPerqBytes, "reduction scratch");
@@ -145,14 +154,19 @@ __global__ void __launch_bounds__(kThreads, 1) pointnet_pass_kernel(const PassPa
     float* s_bias = reinterpret_cast<float*>(smem + C::kOffBias);
     const int tid = threadIdx.x, wg = tid >> 7, t = tid & 127, lane = tid & 31, q4 = lane & 3;
     const int r0 = (t >> 5) * 16 + (lane >> 2);                          // fragment rows r0, r0 + 8
-    const int part = blockIdx.x % C::kSplit;                             // which 128-channel chunks this CTA owns
+    const int part = blockIdx.x % C::kSplit;                             // which 128-channel chunks this CTA owns (fp16: its cluster rank)
     const int stream = blockIdx.x / C::kSplit, nstreams = gridDim.x / C::kSplit;
     const int nq = (p.B > stream) ? (p.B - stream + nstreams - 1) / nstreams : 0;   // queries of this CTA
     const int tpq = p.tiles_per_query;
+    // the fp16 kernel runs the loops over the mid layers to their fixed maximum of three so that they unroll and mid_off
+    // stays in registers (with the CTA pair exchange, ptxas otherwise gives it a stack frame)
     uint32_t mid_off[3] = {0, 0, 0};
     {
         uint32_t o = 0;
-        for (int l = 0; l < p.num_mid; ++l) { mid_off[l] = o; o += (uint32_t)p.mid_N[l] * 128u * C::kMidScale; }
+        for (int l = 0; l < (PRECISE ? p.num_mid : 3); ++l) {
+            if (!PRECISE && l >= p.num_mid) break;
+            mid_off[l] = o; o += (uint32_t)p.mid_N[l] * 128u * C::kMidScale;
+        }
     }
 
     // ---- resident weights: this CTA's W3 chunks, the mid layers shared by every query, the biases
@@ -160,7 +174,8 @@ __global__ void __launch_bounds__(kThreads, 1) pointnet_pass_kernel(const PassPa
         const uint4* src = reinterpret_cast<const uint4*>(p.w3_img + (size_t)part * C::kW3Bytes);
         uint4* dst = reinterpret_cast<uint4*>(smem);
         for (uint32_t i = tid; i < C::kW3Bytes / 16; i += kThreads) dst[i] = src[i];
-        for (int l = 0; l < p.num_mid; ++l) {
+        for (int l = 0; l < (PRECISE ? p.num_mid : 3); ++l) {
+            if (!PRECISE && l >= p.num_mid) break;
             if (l == p.perq_layer) continue;
             const uint4* s = reinterpret_cast<const uint4*>(p.mid_img[l]);
             uint4* d = reinterpret_cast<uint4*>(smem + C::kOffMid + mid_off[l]);
@@ -175,8 +190,20 @@ __global__ void __launch_bounds__(kThreads, 1) pointnet_pass_kernel(const PassPa
         }
         for (int i = tid; i < 64; i += kThreads) s_bias[256 + i] = p.b0[i];
     }
+    uint64_t* xbar = reinterpret_cast<uint64_t*>(smem + C::kOffXBar);   // [wg][full, empty]
+    if (!PRECISE && tid == 0) {
+        // full: one arrival (this CTA arms it for the slot's bytes) plus the peer's asynchronous stores; empty: the peer's
+        // 128 threads once they have read what this CTA stored
+        for (int w = 0; w < kWG; ++w) {
+            mbar_init(xbar + 2 * w, 1);
+            mbar_arrive_expect_tx(xbar + 2 * w, C::kSlotBytes);
+            mbar_init(xbar + 2 * w + 1, 128);
+        }
+        fence_mbar_init();
+    }
     fence_proxy_async_smem();
     __syncthreads();
+    if (!PRECISE) cluster_sync();                 // the peer's barriers are initialised before any remote arrive
 
     uint8_t* wsm = smem + C::kOffWg + wg * C::kWgBytes;
     uint8_t* perq = wsm;
@@ -192,6 +219,14 @@ __global__ void __launch_bounds__(kThreads, 1) pointnet_pass_kernel(const PassPa
         dsc_mid[l] = make_smem_desc(pq ? smem_u32(perq) : smem_u32(smem + C::kOffMid) + mid_off[l], 128, 1024);
         dsc_mid_lo[l] = dsc_mid[l] + (uint64_t)((pq ? 8192u : (uint32_t)p.mid_N[l] * 128u) >> 4);   // lo image follows hi
     }
+    // CTA pair exchange of this warpgroup: the k-th 16 B of thread t's A fragments go to byte 16 (128 k + t) of the slot,
+    // so consecutive threads touch consecutive 16 B.  Running counts of the tiles sent and received give the barrier
+    // parities: the n-th tile received completes phase n of full, the peer's read of the n-th tile sent phase n of empty.
+    uint8_t* slot = smem + C::kOffSlot + wg * C::kSlotBytes;
+    uint64_t* full = xbar + 2 * wg;
+    uint64_t* empty = xbar + 2 * wg + 1;
+    const uint32_t peer = (uint32_t)part ^ 1u;
+    uint32_t nsend = 0, nrecv = 0;
 
     for (int qi = wg; qi < nq; qi += kWG) {
         const size_t q = (size_t)stream + (size_t)qi * nstreams;
@@ -219,71 +254,98 @@ __global__ void __launch_bounds__(kThreads, 1) pointnet_pass_kernel(const PassPa
         float vmax[4 * C::kChunks];
 #pragma unroll
         for (int i = 0; i < 4 * C::kChunks; ++i) vmax[i] = -INFINITY;
-        for (int tq = 0; tq < tpq; ++tq) {
-            // ---- first layer (fp32 FMA): points r0, r0 + 8 of the tile, channels 16 kk + 8 hc + 2 q4 + {0, 1}
-            const int sgi = tq < p.seg[0].tiles ? 0 : 1;
-            const Seg& sg = p.seg[sgi];
-            float cx = 0.f, cy = 0.f, cz = 0.f;
-            if (sg.center) { cx = p.query[q * 3 + 0]; cy = p.query[q * 3 + 1]; cz = p.query[q * 3 + 2]; }
-            float px[2], py[2], pz[2];
+        // fp16: step 2k produces this CTA's tile of the pair (2k, 2k + 1), step 2k + 1 receives the peer's; of a pair with
+        // one tile, the CTA that owns it produces it and the other only receives.  Which tile of a pair a CTA owns
+        // alternates per query (and between the warpgroups), so odd tile totals balance over the pair.
+        const int own = PRECISE ? 0 : (part ^ wg ^ (qi >> 1)) & 1;
+        for (int i = 0; i < tpq; ++i) {
+            const int tq = PRECISE ? i : (i & ~1) + own;
+            const bool mine = PRECISE || (!(i & 1) && tq < tpq);
+            uint32_t a2[8][4], a2l[8][kL];                // the tile's 128 activations: A fragments of the big layer's 8 k-steps
+            if (mine) {
+                // ---- first layer (fp32 FMA): points r0, r0 + 8 of the tile, channels 16 kk + 8 hc + 2 q4 + {0, 1}
+                const int sgi = tq < p.seg[0].tiles ? 0 : 1;
+                const Seg& sg = p.seg[sgi];
+                float cx = 0.f, cy = 0.f, cz = 0.f;
+                if (sg.center) { cx = p.query[q * 3 + 0]; cy = p.query[q * 3 + 1]; cz = p.query[q * 3 + 2]; }
+                float px[2], py[2], pz[2];
 #pragma unroll
-            for (int h = 0; h < 2; ++h) {
-                int local = (tq - (sgi ? p.seg[0].tiles : 0)) * kTile + r0 + 8 * h;
-                if (local >= sg.n) local = 0;                              // duplicate padding
-                const float* src = sg.ptr + (q * sg.n + local) * 3;
-                px[h] = src[0] - cx; py[h] = src[1] - cy; pz[h] = src[2] - cz;   // model.py:303
-            }
-            uint32_t a[4][4], al[4][kL];
+                for (int h = 0; h < 2; ++h) {
+                    int local = (tq - (sgi ? p.seg[0].tiles : 0)) * kTile + r0 + 8 * h;
+                    if (local >= sg.n) local = 0;                              // duplicate padding
+                    const float* src = sg.ptr + (q * sg.n + local) * 3;
+                    px[h] = src[0] - cx; py[h] = src[1] - cy; pz[h] = src[2] - cz;   // model.py:303
+                }
+                uint32_t a[4][4], al[4][kL];
 #pragma unroll
-            for (int kk = 0; kk < 4; ++kk) {
+                for (int kk = 0; kk < 4; ++kk) {
 #pragma unroll
-                for (int hc = 0; hc < 2; ++hc) {
-                    const int ch = kk * 16 + hc * 8 + 2 * q4;
-                    const float2 wx = *reinterpret_cast<const float2*>(wq + 0 * 64 + ch);
-                    const float2 wy = *reinterpret_cast<const float2*>(wq + 1 * 64 + ch);
-                    const float2 wz = *reinterpret_cast<const float2*>(wq + 2 * 64 + ch);
-                    const float2 bb = *reinterpret_cast<const float2*>(s_b0 + ch);
+                    for (int hc = 0; hc < 2; ++hc) {
+                        const int ch = kk * 16 + hc * 8 + 2 * q4;
+                        const float2 wx = *reinterpret_cast<const float2*>(wq + 0 * 64 + ch);
+                        const float2 wy = *reinterpret_cast<const float2*>(wq + 1 * 64 + ch);
+                        const float2 wz = *reinterpret_cast<const float2*>(wq + 2 * 64 + ch);
+                        const float2 bb = *reinterpret_cast<const float2*>(s_b0 + ch);
 #pragma unroll
-                    for (int h = 0; h < 2; ++h) {
-                        // same association as the fp32 path: fma(wx, x, fma(wy, y, fma(wz, z, b)))
-                        const float v0 = fmaf(wx.x, px[h], fmaf(wy.x, py[h], fmaf(wz.x, pz[h], bb.x)));
-                        const float v1 = fmaf(wx.y, px[h], fmaf(wy.y, py[h], fmaf(wz.y, pz[h], bb.y)));
-                        pack_act<PRECISE>(v0, v1, a[kk][hc * 2 + h], al[kk][PRECISE ? hc * 2 + h : 0]);
+                        for (int h = 0; h < 2; ++h) {
+                            // same association as the fp32 path: fma(wx, x, fma(wy, y, fma(wz, z, b)))
+                            const float v0 = fmaf(wx.x, px[h], fmaf(wy.x, py[h], fmaf(wz.x, pz[h], bb.x)));
+                            const float v1 = fmaf(wx.y, px[h], fmaf(wy.y, py[h], fmaf(wz.y, pz[h], bb.y)));
+                            pack_act<PRECISE>(v0, v1, a[kk][hc * 2 + h], al[kk][PRECISE ? hc * 2 + h : 0]);
+                        }
                     }
                 }
-            }
-            // ---- mid layers: 64 -> 64 ..., then 64 -> 128 into the big layer's A fragments; A stays in registers
-            const float* bl = s_bias;
+                // ---- mid layers: 64 -> 64 ..., then 64 -> 128 into the big layer's A fragments; A stays in registers
+                const float* bl = s_bias;
 #pragma unroll
-            for (int l = 0; l < 2; ++l) {
-                if (l >= p.num_mid - 1) break;
-                float d[32];
+                for (int l = 0; l < 2; ++l) {
+                    if (l >= p.num_mid - 1) break;
+                    float d[32];
 #pragma unroll
-                for (int i = 0; i < 32; ++i) d[i] = 0.f;
-                wgmma_fence();
+                    for (int i = 0; i < 32; ++i) d[i] = 0.f;
+                    wgmma_fence();
 #pragma unroll
-                for (int ks = 0; ks < 4; ++ks)
-                    mid_mma<PRECISE>(d, a[ks], reinterpret_cast<const uint32_t (&)[4]>(al[PRECISE ? ks : 0]), dsc_mid[l] + (uint64_t)(ks * 16), dsc_mid_lo[l] + (uint64_t)(ks * 16), ks > 0);
-                wgmma_commit();
-                wgmma_wait<0>();
-                fence_regs(d);
-                pack_acc<PRECISE>(d, bl, q4, a, al);
-                bl += 64;
-            }
-            uint32_t a2[8][4], a2l[8][kL];                // the tile's 128 activations: A fragments of the big layer's 8 k-steps
-            {
-                const uint64_t w = p.num_mid == 3 ? dsc_mid[2] : dsc_mid[0], w_lo = p.num_mid == 3 ? dsc_mid_lo[2] : dsc_mid_lo[0];
-                float d[64];
+                    for (int ks = 0; ks < 4; ++ks)
+                        mid_mma<PRECISE>(d, a[ks], reinterpret_cast<const uint32_t (&)[4]>(al[PRECISE ? ks : 0]), dsc_mid[l] + (uint64_t)(ks * 16), dsc_mid_lo[l] + (uint64_t)(ks * 16), ks > 0);
+                    wgmma_commit();
+                    wgmma_wait<0>();
+                    fence_regs(d);
+                    pack_acc<PRECISE>(d, bl, q4, a, al);
+                    bl += 64;
+                }
+                {
+                    const uint64_t w = p.num_mid == 3 ? dsc_mid[2] : dsc_mid[0], w_lo = p.num_mid == 3 ? dsc_mid_lo[2] : dsc_mid_lo[0];
+                    float d[64];
 #pragma unroll
-                for (int i = 0; i < 64; ++i) d[i] = 0.f;
-                wgmma_fence();
+                    for (int i = 0; i < 64; ++i) d[i] = 0.f;
+                    wgmma_fence();
 #pragma unroll
-                for (int ks = 0; ks < 4; ++ks)
-                    mid_mma<PRECISE>(d, a[ks], reinterpret_cast<const uint32_t (&)[4]>(al[PRECISE ? ks : 0]), w + (uint64_t)(ks * 16), w_lo + (uint64_t)(ks * 16), ks > 0);
-                wgmma_commit();
-                wgmma_wait<0>();
-                fence_regs(d);
-                pack_acc<PRECISE>(d, bl, q4, a2, a2l);
+                    for (int ks = 0; ks < 4; ++ks)
+                        mid_mma<PRECISE>(d, a[ks], reinterpret_cast<const uint32_t (&)[4]>(al[PRECISE ? ks : 0]), w + (uint64_t)(ks * 16), w_lo + (uint64_t)(ks * 16), ks > 0);
+                    wgmma_commit();
+                    wgmma_wait<0>();
+                    fence_regs(d);
+                    pack_acc<PRECISE>(d, bl, q4, a2, a2l);
+                }
+                if (!PRECISE) {
+                    // ---- send: once the peer has read the previous tile out of its slot, write this one there
+                    if (nsend > 0) mbar_wait_cluster_bounded(empty, (nsend - 1) & 1);
+                    const uint32_t dst = mapa(smem_u32(slot), peer) + 16u * (uint32_t)t, bar = mapa(smem_u32(full), peer);
+#pragma unroll
+                    for (int k = 0; k < 8; ++k) st_async_v4(dst + 2048u * k, a2[k], bar);
+                    ++nsend;
+                }
+            } else {
+                // ---- receive the peer's tile: the same registers it packed, then release the slot
+                mbar_wait_cluster_bounded(full, nrecv & 1);
+#pragma unroll
+                for (int k = 0; k < 8; ++k) {
+                    const uint4 v = reinterpret_cast<const uint4*>(slot)[128 * k + t];
+                    a2[k][0] = v.x; a2[k][1] = v.y; a2[k][2] = v.z; a2[k][3] = v.w;
+                }
+                mbar_arrive_cluster(mapa(smem_u32(empty), peer));
+                if (t == 0) mbar_arrive_expect_tx(full, C::kSlotBytes);    // arm the next phase: the peer's next tile
+                ++nrecv;
             }
             // ---- big layer 128 -> this CTA's channels: D[64 points][128 channels] per chunk, max over the points.  Unrolled,
             // ptxas overlaps one chunk's reduction with the next chunk's MMAs (two accumulators); the precise variant's
@@ -353,6 +415,7 @@ __global__ void __launch_bounds__(kThreads, 1) pointnet_pass_kernel(const PassPa
             *reinterpret_cast<float4*>(p.out + q * 1024 + (size_t)(part * kC + 4 * i)) = v;
         }
     }
+    if (!PRECISE) cluster_sync();                 // no CTA exits while its peer may still write its slots or arrive on its barriers
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -513,6 +576,7 @@ struct TcWeights {
     bool fc_on_tc = true;
     std::vector<void*> allocs;
     int sm_count = 132;
+    int pass_clusters = 66;      // query streams of pointnet_pass_kernel<false>: CTA-pair clusters that are co-resident
     // profile of the dominant kernel (bench.py roofline)
     bool prof_on = false;
     std::vector<std::pair<cudaEvent_t, cudaEvent_t>> prof_events;
@@ -552,6 +616,22 @@ uint8_t* pack_w3(TcWeights& t, const Layer& L, bool split = false) {   // 8 chun
     return img;
 }
 
+// launch configuration of pointnet_pass_kernel<false>: CTA 2j and 2j + 1 (one query stream) form a cluster of two
+cudaLaunchConfig_t pass_cluster_config(int grid, cudaStream_t st, cudaLaunchAttribute (&attr)[1]) {
+    cudaLaunchConfig_t cfg{};
+    cfg.gridDim = dim3((unsigned)grid);
+    cfg.blockDim = dim3(kThreads);
+    cfg.dynamicSmemBytes = Cfg<false>::kSmemBytes;
+    cfg.stream = st;
+    attr[0].id = cudaLaunchAttributeClusterDimension;
+    attr[0].val.clusterDim.x = 2;
+    attr[0].val.clusterDim.y = 1;
+    attr[0].val.clusterDim.z = 1;
+    cfg.attrs = attr;
+    cfg.numAttrs = 1;
+    return cfg;
+}
+
 void launch_pass(Model& m, const TcStack& s, const Seg& s0, const Seg& s1, const float* query, const float* R,
                  int64_t B, int perq_layer, const uint8_t* perq_img, float* out, cudaStream_t st, bool precise) {
     PassParams p{};
@@ -570,7 +650,7 @@ void launch_pass(Model& m, const TcStack& s, const Seg& s0, const Seg& s1, const
         P2S_CHECK(s.mid_N[l] == (l == s.num_mid - 1 ? 128 : 64), "pass kernel: mid layers must be 64 -> 64 ... -> 128");
     TcWeights& t = *m.tc;
     const int split = precise ? Cfg<true>::kSplit : Cfg<false>::kSplit;
-    int streams = t.sm_count / split;
+    int streams = precise ? t.sm_count / split : t.pass_clusters;
     if ((int64_t)streams > B) streams = (int)B;
     const int grid = streams * split;
     cudaEvent_t e0 = nullptr, e1 = nullptr;
@@ -580,7 +660,12 @@ void launch_pass(Model& m, const TcStack& s, const Seg& s0, const Seg& s1, const
         P2S_CUDA(cudaEventRecord(e0, st));
     }
     if (precise) P2S_LAUNCH(pointnet_pass_kernel<true>, grid, kThreads, Cfg<true>::kSmemBytes, st, p);
-    else P2S_LAUNCH(pointnet_pass_kernel<false>, grid, kThreads, Cfg<false>::kSmemBytes, st, p);
+    else {
+        cudaLaunchAttribute cluster[1];
+        const cudaLaunchConfig_t cfg = pass_cluster_config(grid, st, cluster);
+        P2S_CUDA(cudaLaunchKernelEx(&cfg, pointnet_pass_kernel<false>, p));
+        g_launches.fetch_add(1, std::memory_order_relaxed);
+    }
     if (prof) {
         P2S_CUDA(cudaEventRecord(e1, st));
         t.prof_events.emplace_back(e0, e1);
@@ -629,6 +714,16 @@ void tc_build(Model& m) {
     t->sm_count = prop.multiProcessorCount;
     P2S_CUDA(cudaFuncSetAttribute(pointnet_pass_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Cfg<false>::kSmemBytes));
     P2S_CUDA(cudaFuncSetAttribute(pointnet_pass_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Cfg<true>::kSmemBytes));
+    {
+        // one wave: no more streams than clusters of two that fit on the device at once (both CTAs of a cluster run on
+        // SMs of the same GPC)
+        cudaLaunchAttribute cluster[1];
+        const cudaLaunchConfig_t cfg = pass_cluster_config(2 * (t->sm_count / 2), 0, cluster);
+        int clusters = 0;
+        P2S_CUDA(cudaOccupancyMaxActiveClusters(&clusters, pointnet_pass_kernel<false>, &cfg));
+        P2S_CHECK(clusters > 0, "pass kernel: no cluster of two CTAs fits on the device");
+        t->pass_clusters = std::min(clusters, t->sm_count / 2);
+    }
     auto build_stn = [&](TcStack& s, const Stn& stn, const Layer* c0a, const Layer* c0b) {
         // QSTN: x -> conv1(3->64) [layer 0] -> conv2 (64->128) -> conv3 ; STN64 on feat: conv0a [layer 0] -> conv0b -> conv1 -> conv2 -> conv3
         if (!c0a) {

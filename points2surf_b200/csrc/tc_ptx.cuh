@@ -1,5 +1,5 @@
-// Thin inline-PTX wrappers for the Hopper (sm_90a) tensor-core path: mbarrier, bulk async copy (TMA 1-D),
-// warpgroup MMA (wgmma) with shared-memory matrix descriptors.
+// Thin inline-PTX wrappers for the Hopper (sm_90a) tensor-core path: mbarrier, thread-block clusters, bulk async copy
+// (TMA 1-D), warpgroup MMA (wgmma) with shared-memory matrix descriptors.
 // Bit layouts follow the PTX ISA "Asynchronous Warpgroup Level Matrix Multiply-Accumulate" chapter.
 #pragma once
 #include <cstdint>
@@ -49,6 +49,44 @@ __device__ __forceinline__ bool mbar_test_wait(uint64_t* bar, uint32_t parity) {
 }
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
     while (!mbar_try_wait(bar, parity)) {}
+}
+
+// ---------------------------------------------------------------- thread-block clusters (distributed shared memory)
+// shared::cta address -> the shared::cluster address of the same offset in CTA `rank` of the cluster
+__device__ __forceinline__ uint32_t mapa(uint32_t addr, uint32_t rank) {
+    uint32_t r;
+    asm("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(addr), "r"(rank));
+    return r;
+}
+// every thread of every CTA of the cluster: prior shared-memory writes and barrier inits are visible cluster-wide after it
+__device__ __forceinline__ void cluster_sync() {
+    asm volatile("barrier.cluster.arrive.release;\n\tbarrier.cluster.wait.acquire;" ::: "memory");
+}
+// asynchronous 16-byte store into the shared memory of another CTA of the cluster; its completion counts 16 bytes of the
+// transaction count of that CTA's mbarrier `bar_addr` (both shared::cluster addresses), released at cluster scope
+__device__ __forceinline__ void st_async_v4(uint32_t addr, const uint32_t (&v)[4], uint32_t bar_addr) {
+    asm volatile("st.async.shared::cluster.mbarrier::complete_tx::bytes.v4.b32 [%0], {%1, %2, %3, %4}, [%5];"
+                 ::"r"(addr), "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(bar_addr) : "memory");
+}
+// arrive on an mbarrier of any CTA of the cluster (shared::cluster address), releasing this thread's prior accesses
+__device__ __forceinline__ void mbar_arrive_cluster(uint32_t bar_addr) {
+    asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(bar_addr) : "memory");
+}
+// wait on a local mbarrier whose arrivals come from other CTAs of the cluster: acquires what they released
+__device__ __forceinline__ bool mbar_try_wait_cluster(uint64_t* bar, uint32_t parity) {
+    uint32_t ok;
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "mbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 p, [%1], %2;\n\t"
+        "selp.u32 %0, 1, 0, p;\n\t}"
+        : "=r"(ok) : "r"(smem_u32(bar)), "r"(parity) : "memory");
+    return ok != 0;
+}
+__device__ __forceinline__ void mbar_wait_cluster_bounded(uint64_t* bar, uint32_t parity) {
+    long long t0 = clock64();
+    while (!mbar_try_wait_cluster(bar, parity)) {
+        if (clock64() - t0 > 2000000000LL) __trap();
+    }
 }
 
 __device__ __forceinline__ bool elect_one() {
