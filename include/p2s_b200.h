@@ -558,6 +558,31 @@ int p2s_op_bn_maxpool_fwd(const float* z, int64_t B, int npts, int C, const floa
 int p2s_op_bn_maxpool_bwd(const float* dout, const int32_t* arg, const float* out, const float* z, int64_t B,
                           int npts, int C, const float* mean, const float* invstd, const float* gamma, int relu,
                           double* s1, double* s2, float* dz, void* stream);
+/* Eval-mode backward (model.eval(): BatchNorm with mean = running_mean, invstd = 1/sqrt(running_var + eps), constants of
+ * the backward, so every row is independent and nothing needs a second pass).
+ * BatchNorm(eval)(+ReLU), one pass over the M rows: g = dy masked by y > 0 (y = forward output, NULL without ReLU),
+ * dz = gamma invstd g [M, C]; dbeta = sum g, dgamma = sum g (z - mean) invstd, dbias = sum dz (the gradient of the bias of
+ * the layer in front), f64 [C] each, overwritten.
+ * Per element, with the f64 sums' rounding negligible: |dz - exact| <= 2u |dz|, |dgamma - exact| <= 2u sum |g xhat| +
+ * u |dgamma|, |dbias - exact| <= 2u sum |dz| + u |dbias| (u = 2^-24; the last u is the caller's conversion to fp32). */
+int p2s_op_bn_eval_backward(const float* dy, const float* z, const float* y, int64_t M, int C, const float* mean,
+                            const float* invstd, const float* gamma, double* dbeta, double* dgamma, double* dbias,
+                            float* dz, void* stream);
+/* BatchNorm(eval)(+ReLU) + max over the npts points, fused with the conv in front of it (z = x W^T + bias, x [B*npts, K],
+ * W [C, K], C <= 4096): the backward from dout [B, C] given the forward's arg [B, C] (p2s_op_bn_maxpool_fwd with the
+ * running statistics; arg taken on the normalised values, first maximum) and out [B, C] (read for the ReLU mask only,
+ * may be NULL without ReLU).  Only the arg row of each (query, channel) carries a gradient, dz[b,c] = gamma invstd
+ * dout[b,c] (0 where out <= 0 under ReLU); the dense [B*npts, C] gradient is never formed:
+ *     dW[c,:] += sum_b dz[b,c] x[b*npts + arg[b,c], :]                  (gather over B rows, fp32 FMA + fp32 atomics;
+ *                                                                       every row is read, so 0 * Inf gives NaN like the dense path)
+ *     dx[b*npts + i, :] = sum_{c : arg[b,c] = i} dz[b,c] W[c,:]        (scatter, ascending c, every row written; NULL: skipped)
+ *     dbias = sum_b dz, dgamma = sum_b g xhat(arg row), dbeta = sum_b g  (f64 [C], overwritten)
+ * dW and dx are within gamma_n sum |dz| |x| (resp. |W|) of the exact sums of the rounded dz (n = terms + 2).  All row
+ * offsets are 64-bit, so B * npts * K may exceed 2^31. */
+int p2s_op_bn_maxpool_eval_bwd(const float* dout, const int32_t* arg, const float* out, const float* z, const float* x,
+                               const float* W, int64_t B, int npts, int C, int K, const float* mean, const float* invstd,
+                               const float* gamma, int relu, float* dW, double* dbias, double* dgamma, double* dbeta,
+                               float* dx, void* stream);
 /* MaxPool1d over the npts points of each query: y [B, npts, C] -> out [B, C], arg [B, C] (first maximum) */
 int p2s_op_maxpool_fwd(const float* y, int64_t B, int npts, int C, float* out, int32_t* arg, void* stream);
 int p2s_op_maxpool_bwd(const float* dout, const int32_t* arg, int64_t B, int npts, int C, float* dy, void* stream);

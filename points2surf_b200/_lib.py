@@ -107,6 +107,9 @@ SIGNATURES = {
     'p2s_op_bn_backward': (C.c_int, [_vp, _vp, _vp, _i64, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     'p2s_op_bn_maxpool_fwd': (C.c_int, [_vp, _i64, _i32, _i32, _vp, _vp, _vp, _vp, _i32, _vp, _vp, _vp]),
     'p2s_op_bn_maxpool_bwd': (C.c_int, [_vp, _vp, _vp, _vp, _i64, _i32, _i32, _vp, _vp, _vp, _i32, _vp, _vp, _vp, _vp]),
+    'p2s_op_bn_eval_backward': (C.c_int, [_vp, _vp, _vp, _i64, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    'p2s_op_bn_maxpool_eval_bwd': (C.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _i64, _i32, _i32, _i32, _vp, _vp, _vp, _i32, _vp, _vp,
+                                             _vp, _vp, _vp, _vp]),
     'p2s_op_maxpool_fwd': (C.c_int, [_vp, _i64, _i32, _i32, _vp, _vp, _vp]),
     'p2s_op_maxpool_bwd': (C.c_int, [_vp, _vp, _i64, _i32, _i32, _vp, _vp]),
     'p2s_op_loss': (C.c_int, [_vp, _vp, _vp, _vp, _i64, _f32, _f32, _i32, _vp, _vp, _vp]),

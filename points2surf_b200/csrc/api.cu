@@ -634,6 +634,19 @@ P2S_OP(p2s_op_bn_maxpool_bwd, (const float* dout, const int32_t* arg, const floa
                                float* dz, void* stream),
        P2S_CHECK(dout && arg && out && z && mean && invstd && gamma && s1 && s2 && dz && npts > 0, "bad argument");
         op_bn_maxpool_bwd(dout, arg, out, z, B, npts, C, mean, invstd, gamma, relu != 0, s1, s2, dz, as_stream(stream)))
+P2S_OP(p2s_op_bn_eval_backward, (const float* dy, const float* z, const float* y, int64_t M, int C, const float* mean,
+                                 const float* invstd, const float* gamma, double* dbeta, double* dgamma, double* dbias, float* dz,
+                                 void* stream),
+       P2S_CHECK(dy && z && mean && invstd && gamma && dbeta && dgamma && dbias && dz, "null argument");
+        op_bn_eval_backward(dy, z, y, M, C, mean, invstd, gamma, dbeta, dgamma, dbias, dz, as_stream(stream)))
+P2S_OP(p2s_op_bn_maxpool_eval_bwd, (const float* dout, const int32_t* arg, const float* out, const float* z, const float* x,
+                                    const float* W, int64_t B, int npts, int C, int K, const float* mean, const float* invstd,
+                                    const float* gamma, int relu, float* dW, double* dbias, double* dgamma, double* dbeta,
+                                    float* dx, void* stream),
+       P2S_CHECK(dout && arg && (out || !relu) && z && x && W && mean && invstd && gamma && dW && dbias && dgamma && dbeta &&
+                 npts > 0, "bad argument");
+        op_bn_maxpool_eval_bwd(dout, arg, out, z, x, W, B, npts, C, K, mean, invstd, gamma, relu != 0, dW, dbias, dgamma, dbeta,
+                               dx, as_stream(stream)))
 P2S_OP(p2s_op_maxpool_fwd, (const float* y, int64_t B, int npts, int C, float* out, int32_t* arg, void* stream),
        P2S_CHECK(y && out && arg && npts > 0, "bad argument"); op_maxpool_fwd(y, B, npts, C, out, arg, as_stream(stream)))
 P2S_OP(p2s_op_maxpool_bwd, (const float* dout, const int32_t* arg, int64_t B, int npts, int C, float* dy, void* stream),

@@ -169,6 +169,13 @@ void op_bn_maxpool_fwd(const float* z, int64_t B, int npts, int C, const float* 
 void op_bn_maxpool_bwd(const float* dout, const int32_t* arg, const float* out, const float* z, int64_t B, int npts, int C,
                        const float* mean, const float* invstd, const float* gamma, bool relu, double* s1, double* s2,
                        float* dz, cudaStream_t st);
+void op_bn_eval_backward(const float* dy, const float* z, const float* y_or_null, int64_t M, int C, const float* mean,
+                         const float* invstd, const float* gamma, double* dbeta, double* dgamma, double* dbias, float* dz,
+                         cudaStream_t st);
+void op_bn_maxpool_eval_bwd(const float* dout, const int32_t* arg, const float* out, const float* z, const float* x,
+                            const float* W, int64_t B, int npts, int C, int K, const float* mean, const float* invstd,
+                            const float* gamma, bool relu, float* dW, double* dbias, double* dgamma, double* dbeta,
+                            float* dx, cudaStream_t st);
 void op_maxpool_fwd(const float* y, int64_t B, int npts, int C, float* out, int32_t* arg, cudaStream_t st);
 void op_maxpool_bwd(const float* dout, const int32_t* arg, int64_t B, int npts, int C, float* dy, cudaStream_t st);
 void op_loss(const float* pred, const float* target_mag, const float* radius, const float* target_sign, int64_t B,

@@ -280,6 +280,150 @@ bn_maxpool_bwd_apply_kernel(const float* __restrict__ dout, const int32_t* __res
     }
 }
 
+// ---- eval-mode BatchNorm (running statistics, constant in the backward): every row is independent, so dz, the column
+// sums and the conv3 gradients need no second pass and no dense [rows, C] tensor
+// g = dy masked by the ReLU, dz = gamma invstd g; dbeta += sum g, dgamma += sum g xhat, dbias += sum dz (f64)
+__global__ void __launch_bounds__(256)
+bn_eval_bwd_kernel(const float* __restrict__ dy, const float* __restrict__ z, const float* __restrict__ y, int64_t M,
+                   int C, int64_t rows_per_block, const float* __restrict__ mean, const float* __restrict__ invstd,
+                   const float* __restrict__ gamma, double* __restrict__ dbeta, double* __restrict__ dgamma,
+                   double* __restrict__ dbias, float* __restrict__ dz) {
+    const int c = blockIdx.x * blockDim.x + threadIdx.x;
+    double a1 = 0.0, a2 = 0.0, a3 = 0.0;
+    if (c < C) {
+        const float is = invstd[c], mu = mean[c], gi = gamma[c] * is;
+        const int64_t r0 = (int64_t)blockIdx.y * rows_per_block, r1 = min(M, r0 + rows_per_block);
+#pragma unroll 4
+        for (int64_t r = r0 + threadIdx.y; r < r1; r += blockDim.y) {
+            const int64_t e = r * C + c;
+            float g = dy[e];
+            if (y && !(y[e] > 0.f)) g = 0.f;
+            const float d = gi * g;
+            dz[e] = d;
+            a1 += (double)g;
+            a2 = fma((double)g, (double)((z[e] - mu) * is), a2);
+            a3 += (double)d;
+        }
+    }
+    __shared__ double r[3][256];
+    const int t = threadIdx.y * blockDim.x + threadIdx.x;
+    r[0][t] = a1; r[1][t] = a2; r[2][t] = a3;
+    __syncthreads();
+    if (threadIdx.y == 0 && c < C) {
+        double d1 = 0.0, d2 = 0.0, d3 = 0.0;
+        for (int j = 0; j < (int)blockDim.y; ++j) {
+            const int u = j * blockDim.x + threadIdx.x;
+            d1 += r[0][u]; d2 += r[1][u]; d3 += r[2][u];
+        }
+        atomicAdd(dbeta + c, d1);
+        atomicAdd(dgamma + c, d2);
+        atomicAdd(dbias + c, d3);
+    }
+}
+
+// The conv3 layers in eval mode: z = x W^T + bias, y = act(BN_eval(z)), out = max over the npts points.  Only the arg
+// row of each (query, channel) carries a gradient, dz[b,c] = gamma invstd dout[b,c] (0 where out <= 0 under ReLU).
+// Weight gradient as a gather, one warp per channel over a range of queries, lanes over K:
+//   dW[c,:] += sum_b dz[b,c] x[b*npts + arg[b,c], :]      (fp32 FMA, ranges of queries added with fp32 atomics)
+// and the column sums dbias = sum_b dz, dgamma = sum_b g xhat(arg row), dbeta = sum_b g in f64.  grid (C / 8, splits).
+__global__ void __launch_bounds__(256)
+bn_maxpool_eval_bwd_w_kernel(const float* __restrict__ dout, const int32_t* __restrict__ arg,
+                             const float* __restrict__ out, const float* __restrict__ z, const float* __restrict__ x,
+                             int64_t B, int npts, int C, int K, int64_t rows_per_split, const float* __restrict__ mean,
+                             const float* __restrict__ invstd, const float* __restrict__ gamma, float* __restrict__ dW,
+                             double* __restrict__ dbias, double* __restrict__ dgamma, double* __restrict__ dbeta) {
+    const int lane = threadIdx.x & 31;
+    const int c = blockIdx.x * 8 + (threadIdx.x >> 5);
+    if (c >= C) return;
+    const int64_t b0 = (int64_t)blockIdx.y * rows_per_split, b1 = min(B, b0 + rows_per_split);
+    const float is = invstd[c], mu = mean[c], gi = gamma[c] * is;
+    double a1 = 0.0, a2 = 0.0, a3 = 0.0;
+    for (int k0 = 0; k0 < K; k0 += 32) {
+        const int k = k0 + lane;
+        float acc = 0.f;
+#pragma unroll 4
+        for (int64_t b = b0; b < b1; ++b) {
+            const int64_t e = b * C + c;
+            float g = dout[e];
+            if (out && !(out[e] > 0.f)) g = 0.f;
+            const float d = gi * g;
+            const int64_t row = b * npts + arg[e];
+            if (k0 == 0 && lane == 0) {
+                a1 += (double)g;
+                a2 = fma((double)g, (double)((z[row * C + c] - mu) * is), a2);
+                a3 += (double)d;
+            }
+            if (k < K) acc = fmaf(d, x[row * K + k], acc);
+        }
+        if (k < K && b1 > b0) atomicAdd(dW + (int64_t)c * K + k, acc);
+    }
+    if (lane == 0 && b1 > b0) {
+        atomicAdd(dbeta + c, a1);
+        atomicAdd(dgamma + c, a2);
+        atomicAdd(dbias + c, a3);
+    }
+}
+
+// Input gradient as a scatter, one CTA per query b:
+//   dx[b*npts + i, :] = sum_{c : arg[b,c] = i} dz[b,c] W[c,:]      (0 for the points no channel picked)
+// The channels are sorted by (arg, c) in shared memory (bitonic, keys arg * Cp + c with Cp = C rounded up to a power of
+// two), so each point's channels form one run found by binary search; each warp writes whole rows of dx, every row
+// exactly once, in a fixed order of the terms: no atomics, no memset, bit-reproducible.
+__global__ void __launch_bounds__(256)
+bn_maxpool_eval_bwd_x_kernel(const float* __restrict__ dout, const int32_t* __restrict__ arg,
+                             const float* __restrict__ out, const float* __restrict__ W, int npts, int C, int Cp, int K,
+                             const float* __restrict__ invstd, const float* __restrict__ gamma, float* __restrict__ dx) {
+    extern __shared__ uint32_t sh[];
+    uint32_t* keys = sh;                               // [Cp]
+    float* sdz = reinterpret_cast<float*>(sh + Cp);    // [C]
+    const int64_t b = blockIdx.x;
+    for (int c = threadIdx.x; c < Cp; c += blockDim.x) {
+        if (c < C) {
+            const int64_t e = b * C + c;
+            float g = dout[e];
+            if (out && !(out[e] > 0.f)) g = 0.f;
+            sdz[c] = (gamma[c] * invstd[c]) * g;
+            keys[c] = (uint32_t)arg[e] * (uint32_t)Cp + (uint32_t)c;
+        } else {
+            keys[c] = 0xFFFFFFFFu;
+        }
+    }
+    __syncthreads();
+    for (int k = 2; k <= Cp; k <<= 1) {
+        for (int j = k >> 1; j > 0; j >>= 1) {
+            for (int i = threadIdx.x; i < Cp; i += blockDim.x) {
+                const int ij = i ^ j;
+                if (ij > i) {
+                    const uint32_t u = keys[i], v = keys[ij];
+                    if ((u > v) == ((i & k) == 0)) { keys[i] = v; keys[ij] = u; }
+                }
+            }
+            __syncthreads();
+        }
+    }
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
+    auto lower_bound = [&](uint32_t v) {
+        int lo = 0, hi = Cp;
+        while (lo < hi) {
+            const int mid = (lo + hi) >> 1;
+            if (keys[mid] < v) lo = mid + 1; else hi = mid;
+        }
+        return lo;
+    };
+    for (int i = warp; i < npts; i += nwarps) {
+        const int lo = lower_bound((uint32_t)i * (uint32_t)Cp), hi = lower_bound((uint32_t)(i + 1) * (uint32_t)Cp);
+        float* row = dx + (b * npts + i) * (int64_t)K;
+        for (int k = lane; k < K; k += 32) {
+            float acc = 0.f;
+            for (int j = lo; j < hi; ++j) {
+                const int c = (int)(keys[j] & (uint32_t)(Cp - 1));
+                acc = fmaf(sdz[c], W[(int64_t)c * K + k], acc);
+            }
+            row[k] = acc;
+        }
+    }
+}
+
 // ---------------------------------------------------------------- max over the points of each query, with argmax
 __global__ void maxpool_fwd_kernel(const float* __restrict__ y, int64_t B, int npts, int C, float* __restrict__ out,
                                    int32_t* __restrict__ arg) {
@@ -628,6 +772,48 @@ void op_bn_maxpool_bwd(const float* dout, const int32_t* arg, const float* out, 
     const int tx = C >= 128 ? 128 : (C >= 64 ? 64 : 32);
     P2S_LAUNCH(bn_maxpool_bwd_apply_kernel, dim3((unsigned)cdiv(C, tx), (unsigned)cdiv(npts, 32), (unsigned)B), tx, 0, st, dout,
                arg, out, z, mean, invstd, gamma, s1, s2, B, npts, C, relu ? 1 : 0, dz);
+}
+
+// eval-mode BatchNorm (+ReLU) backward: dz [M, C]; dbeta, dgamma, dbias f64 [C] (zeroed here)
+void op_bn_eval_backward(const float* dy, const float* z, const float* y_or_null, int64_t M, int C, const float* mean,
+                         const float* invstd, const float* gamma, double* dbeta, double* dgamma, double* dbias, float* dz,
+                         cudaStream_t st) {
+    P2S_CUDA(cudaMemsetAsync(dbeta, 0, sizeof(double) * C, st));
+    P2S_CUDA(cudaMemsetAsync(dgamma, 0, sizeof(double) * C, st));
+    P2S_CUDA(cudaMemsetAsync(dbias, 0, sizeof(double) * C, st));
+    if (M <= 0 || C <= 0) return;
+    dim3 blk, g; int64_t rpb;
+    rowwise_grid(M, C, blk, g, rpb);
+    P2S_LAUNCH(bn_eval_bwd_kernel, g, blk, 0, st, dy, z, y_or_null, M, C, rpb, mean, invstd, gamma, dbeta, dgamma, dbias, dz);
+}
+
+// eval-mode BatchNorm (+ReLU) + max-pool backward fused with the conv in front: dW += gather, dx = scatter (NULL: skipped),
+// dbias, dgamma, dbeta f64 [C] (zeroed here).  out is read for the ReLU mask only.
+void op_bn_maxpool_eval_bwd(const float* dout, const int32_t* arg, const float* out, const float* z, const float* x,
+                            const float* W, int64_t B, int npts, int C, int K, const float* mean, const float* invstd,
+                            const float* gamma, bool relu, float* dW, double* dbias, double* dgamma, double* dbeta,
+                            float* dx, cudaStream_t st) {
+    P2S_CUDA(cudaMemsetAsync(dbias, 0, sizeof(double) * C, st));
+    P2S_CUDA(cudaMemsetAsync(dgamma, 0, sizeof(double) * C, st));
+    P2S_CUDA(cudaMemsetAsync(dbeta, 0, sizeof(double) * C, st));
+    if (B <= 0 || C <= 0 || K <= 0) return;
+    P2S_CHECK(C <= 4096, "bn_maxpool_eval_bwd: at most 4096 channels");
+    int Cp = 1;
+    while (Cp < C) Cp <<= 1;
+    // the scatter's sort keys arg * Cp + c, and the bound (npts) * Cp of the last point's run, fit in 32 bits
+    P2S_CHECK((int64_t)npts * Cp < (int64_t)0xFFFFFFFF, "bn_maxpool_eval_bwd: npts * C too large");
+    const float* mask = relu ? out : nullptr;
+    const int64_t cx = cdiv(C, 8);
+    int64_t splits = std::max<int64_t>(1, std::min<int64_t>(B, cdiv(8 * (int64_t)sm_count(), cx)));
+    splits = std::min<int64_t>(splits, 65535);
+    const int64_t rows = cdiv(B, splits);
+    splits = cdiv(B, rows);
+    P2S_LAUNCH(bn_maxpool_eval_bwd_w_kernel, dim3((unsigned)cx, (unsigned)splits), 256, 0, st, dout, arg, mask, z, x, B, npts,
+               C, K, rows, mean, invstd, gamma, dW, dbias, dgamma, dbeta);
+    if (!dx) return;
+    P2S_CHECK(B <= 0x7FFFFFFF, "bn_maxpool_eval_bwd: batch too large for grid.x");
+    const size_t smem = sizeof(uint32_t) * (size_t)Cp + sizeof(float) * (size_t)C;
+    P2S_LAUNCH(bn_maxpool_eval_bwd_x_kernel, (unsigned)B, 256, smem, st, dout, arg, mask, W, npts, C, Cp, K, invstd, gamma, dx);
 }
 
 }  // namespace p2s

@@ -5,11 +5,24 @@ with or without the DataParallel 'module.' prefix), whose forward runs on the CU
 Supported subset (SURVEY.md section 8b): sym_op='max', single_transformer=False, use_feat_stn=True,
 output_dim 2 (imp_surf_magnitude, imp_surf_sign) or 1 (imp_surf, the regression ablation; forward returns [B, 1]
 logits, evaluated with ops.distance_from_logits).  Anything else raises ValueError like the reference does for unknown options
-(points_to_surf_model.py:175).  Inference only: forward() ignores .train() and always uses running
-BatchNorm statistics (the reference evaluates with .eval(), points_to_surf_eval.py:170).
+(points_to_surf_model.py:175).  forward() ignores .train() and always uses running BatchNorm statistics (the
+reference evaluates with .eval(), points_to_surf_eval.py:170).
+
+Gradients.  In eval mode (`m.eval()`), with grad enabled and some parameter or input requiring grad, the logits carry a
+grad_fn and `backward()` fills `.grad` of every parameter (conv / linear weight and bias, BatchNorm weight and bias) and
+input (patch_pts_ps, pts_sub_sample_ms, imp_surf_query_point_ms) that requires grad, with the gradient of the reference's
+eval-mode network (points_to_surf_model.py:296-352, BatchNorm with running_mean / running_var, eps 1e-5), computed by
+CUDA backward kernels (points2surf_b200.train.EvalGrad).  The logits stay the engine's, bit for bit; the backward
+recomputes the activations in fp32, records that network's ReLU masks and max-pool arg-maxes, and differentiates it.  So
+the gradients are those of the fp32 network, which can differ from a precision='tc' forward's decisions near a ReLU or
+max-pool tie.  The caller's sub-sample is centred in place like the reference's `shape_features -= query`: a leaf
+sub-sample that requires grad raises, a non-leaf one passes its gradient on, and the query receives minus the sum of it.
+Train mode and torch.no_grad() return logits without grad_fn.  Double backward is not supported; train-mode
+(batch-statistics) gradients are points2surf_b200.train.TrainStep's.
 """
 import torch
 import torch.nn as nn
+from torch.autograd.function import once_differentiable
 
 from . import arch
 from . import ops
@@ -90,8 +103,55 @@ class PointsToSurfModel(nn.Module):
         query = x['imp_surf_query_point_ms']
         if not patch.is_cuda:
             raise ops.P2SError('PointsToSurfModel.forward needs CUDA tensors: points2surf_b200 has no CPU path')
+        if not self.training and torch.is_grad_enabled():
+            params = tuple(self.parameters())
+            if any(t.requires_grad for t in (patch, shape, query) + params):
+                if shape.is_leaf and shape.requires_grad:
+                    # what the reference's in-place centring raises (points_to_surf_model.py:303), before any work
+                    raise RuntimeError('a leaf Variable that requires grad is being used in an in-place operation.')
+                out, _ = _EvalForward.apply(self, patch, shape, query, *params)
+                return out
         eng = self._get_engine(patch.device)
         out = eng.forward(patch, shape, query)
         # the reference centres the caller's sub-sample in place (points_to_surf_model.py:303); keep that side effect
         shape -= query.unsqueeze(1).expand(shape.shape)
         return out
+
+
+class _EvalForward(torch.autograd.Function):
+    """Eval-mode forward on the engine + the in-place centring of the sub-sample, differentiable in all inputs and the
+    parameters (passed explicitly, in `model.parameters()` order, so autograd hands their gradients to the Parameters).
+    Keeps references to its inputs only; the backward recomputes the fp32 activations (train.EvalGrad)."""
+
+    @staticmethod
+    def forward(ctx, model, patch, shape, query, *params):
+        out = model._get_engine(patch.device).forward(patch, shape, query)
+        shape -= query.unsqueeze(1).expand(shape.shape)      # the reference's in-place centring (model.py:303)
+        ctx.mark_dirty(shape)
+        if not (shape.requires_grad or query.requires_grad):
+            ctx.mark_non_differentiable(shape)              # like `shape -= query` on two tensors without grad
+        ctx.model = model
+        ctx.save_for_backward(patch, shape, query, *params)
+        return out, shape
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, dout, dshape_out):
+        from .train import EvalGrad
+        m = ctx.model
+        patch, shape, query = ctx.saved_tensors[:3]
+        params = ctx.saved_tensors[3:]
+        sd = dict(zip((n for n, _ in m.named_parameters()), (t.detach() for t in params)))
+        sd.update((n, b.detach()) for n, b in m.named_buffers())
+        eg = EvalGrad(sd, m.use_point_stn, m.shared_transformation, m.num_points, m.sub_sample_size, m.net_size_max,
+                      output_dim=m.output_dim, device=patch.device)
+        # `shape` holds the centred sub-sample (the same fp32 subtraction as the recompute's centring, which a zero
+        # query leaves exact)
+        eg.forward({'patch_pts_ps': patch.detach(), 'pts_sub_sample_ms': shape.detach(),
+                    'imp_surf_query_point_ms': torch.zeros_like(query.detach())})
+        dpatch, dshape, dquery = eg.backward_inputs(dout, dshape_out)
+        grads = eg.named_gradients()
+        need = ctx.needs_input_grad
+        dparams = [grads[n].reshape(t.shape) if need[4 + i] else None
+                   for i, (n, t) in enumerate(zip((n for n, _ in m.named_parameters()), params))]
+        return (None, dpatch if need[1] else None, dshape if need[2] else None, dquery if need[3] else None, *dparams)

@@ -77,6 +77,8 @@ class TrainStep:
         ts.state_dict()                # reference-named tensors (loadable by PointsToSurfModel / Engine)
     """
 
+    _momentum = True     # SGD momentum buffers (EvalGrad, which never steps, has none)
+
     def __init__(self, state_dict, use_point_stn, shared_transformer, points_per_patch=300, sub_sample_size=1000,
                  net_size=1024, lr=0.01, momentum=0.9, device=None, prims=None,
                  outputs=('imp_surf_magnitude', 'imp_surf_sign'), output_loss_weights=None, fixed_radius=False,
@@ -114,7 +116,7 @@ class TrainStep:
         total = sum(int(torch.Size(s).numel()) for _, s in shapes)
         self.flat_params = torch.empty(total, dtype=dtype, device=self.device)
         self.flat_grads = torch.zeros_like(self.flat_params)
-        self.flat_mom = torch.zeros_like(self.flat_params)
+        self.flat_mom = torch.zeros_like(self.flat_params) if self._momentum else None
         self.params, self.grads, self._orig_shape = {}, {}, {}
         off = 0
         for name, shp in shapes:
@@ -145,10 +147,7 @@ class TrainStep:
         t = _Tape()
         t.name, t.bn, t.x, t.z, t.pool, t.relu = name, bn, x, z, None, relu
         if bn is not None:
-            y, t.mean, t.invstd = p.bn_forward(z, self.params[bn + '.weight'], self.params[bn + '.bias'], relu,
-                                               self.buffers[bn + '.running_mean'], self.buffers[bn + '.running_var'],
-                                               BN_EPS, BN_MOMENTUM)
-            self.buffers[bn + '.num_batches_tracked'] += 1
+            y, t.mean, t.invstd = self._bn_fwd(z, bn, relu)
             t.y_mask = y if relu else None
         else:
             if relu:
@@ -162,30 +161,47 @@ class TrainStep:
         materialised (model.py:45-48, 104-107, 203-212)."""
         p = self.p
         z = p.gemm_nt(x, self.params[name + '.weight'], self.params[name + '.bias'])
-        out, arg, mean, invstd = p.bn_maxpool_forward(z, B, n, self.params[bn + '.weight'], self.params[bn + '.bias'], relu,
-                                                      self.buffers[bn + '.running_mean'], self.buffers[bn + '.running_var'],
-                                                      BN_EPS, BN_MOMENTUM)
-        self.buffers[bn + '.num_batches_tracked'] += 1
+        out, arg, mean, invstd = self._bn_pool_fwd(z, bn, relu, B, n)
         t = _Tape()
         t.name, t.bn, t.x, t.z, t.y_mask, t.mean, t.invstd, t.pool, t.relu = name, bn, x, z, None, mean, invstd, (out, arg, B, n), relu
         tape.append(t)
         return out
 
-    def _lin_bwd(self, t, dy, need_dx=True):
+    # train-mode BatchNorm: batch statistics, running statistics updated
+    def _bn_fwd(self, z, bn, relu):
+        y, mean, invstd = self.p.bn_forward(z, self.params[bn + '.weight'], self.params[bn + '.bias'], relu,
+                                            self.buffers[bn + '.running_mean'], self.buffers[bn + '.running_var'],
+                                            BN_EPS, BN_MOMENTUM)
+        self.buffers[bn + '.num_batches_tracked'] += 1
+        return y, mean, invstd
+
+    def _bn_pool_fwd(self, z, bn, relu, B, n):
+        out, arg, mean, invstd = self.p.bn_maxpool_forward(z, B, n, self.params[bn + '.weight'], self.params[bn + '.bias'], relu,
+                                                           self.buffers[bn + '.running_mean'],
+                                                           self.buffers[bn + '.running_var'], BN_EPS, BN_MOMENTUM)
+        self.buffers[bn + '.num_batches_tracked'] += 1
+        return out, arg, mean, invstd
+
+    def _bn_bwd(self, t, dy):
+        """dy -> dz through act + BatchNorm; accumulates the BatchNorm's parameter gradients."""
         p = self.p
         if t.pool is not None:
             out, arg, B, n = t.pool
             dz, dgamma, dbeta = p.bn_maxpool_backward(dy, arg, out, t.z, t.mean, t.invstd, self.params[t.bn + '.weight'], t.relu, B, n)
-        elif t.bn is not None:
+        else:
             dz, dgamma, dbeta = p.bn_backward(dy, t.z, t.y_mask, t.mean, t.invstd, self.params[t.bn + '.weight'])
+        p.axpy_(self.grads[t.bn + '.weight'], dgamma)
+        p.axpy_(self.grads[t.bn + '.bias'], dbeta)
+        # the bias of a layer in front of a train-mode BatchNorm has an identically zero gradient (dz sums to zero
+        # over the rows by construction; torch's value is rounding noise): it stays 0
+        return dz
+
+    def _lin_bwd(self, t, dy, need_dx=True):
+        p = self.p
+        if t.bn is not None:
+            dz = self._bn_bwd(t, dy)
         else:
             dz = dy
-        if t.bn is not None:
-            p.axpy_(self.grads[t.bn + '.weight'], dgamma)
-            p.axpy_(self.grads[t.bn + '.bias'], dbeta)
-            # the bias of a layer in front of a train-mode BatchNorm has an identically zero gradient (dz sums to zero
-            # over the rows by construction; torch's value is rounding noise): it stays 0
-        else:
             p.axpy_(self.grads[t.name + '.bias'], p.col_sum(dz))
         p.gemm_tn(dz, t.x, out=self.grads[t.name + '.weight'])
         if not need_dx:
@@ -283,27 +299,44 @@ class TrainStep:
         self._rec = rec
         return logits
 
-    def backward(self, dlogits):
-        """Accumulates into self.grads (call zero_grad() first, like optimizer.zero_grad())."""
+    def backward(self, dlogits, need_inputs=False):
+        """Accumulates into self.grads (call zero_grad() first, like optimizer.zero_grad()).  need_inputs: also
+        -> (d patch_pts_ps [B,P,3], d centred sub-sample [B,S,3])."""
         p = self.p
         rec = self._rec
         B, head = rec['B'], rec['head']
+        P, S = self.P, self.S
         d = self._lin_bwd(head[4], dlogits.contiguous())
         d = self._lin_bwd(head[3], d)
         d = self._lin_bwd(head[2], d)
         half = self.net // 2
         d_loc, d_glob = d[:, :half].contiguous(), d[:, half:].contiguous()
         need_R = rec['R'] is not None
+        need_dpts = need_R or need_inputs
         dg_loc = self._lin_bwd(head[1], d_loc)
-        dpatch_t = self._feat_bwd(rec['feat_local'], dg_loc, need_R)
+        dpatch_t = self._feat_bwd(rec['feat_local'], dg_loc, need_dpts)
         dg_glob = self._lin_bwd(head[0], d_glob)
-        dsub_t = self._feat_bwd(rec['feat_global'], dg_glob, need_R)
+        dsub_t = self._feat_bwd(rec['feat_global'], dg_glob, need_dpts)
         if need_R:
-            dR = self._rotate_bwd_R(dsub_t, rec['sub'], B, self.S)
-            p.axpy_(dR, self._rotate_bwd_R(dpatch_t, rec['patch'], B, self.P))
+            dR = self._rotate_bwd_R(dsub_t, rec['sub'], B, S)
+            p.axpy_(dR, self._rotate_bwd_R(dpatch_t, rec['patch'], B, P))
             dq = p.quat_to_rot_bwd(rec['qraw'], dR.view(B, 9))
-            self._stn_bwd(rec['qstn'], dq, False)
+            dsrc = self._stn_bwd(rec['qstn'], dq, need_inputs)       # d of the QSTN's input points
         self._rec = None
+        if not need_inputs:
+            return None
+        if not need_R:
+            return dpatch_t.view(B, P, 3), dsub_t.view(B, S, 3)
+        Rt = p.transpose(rec['R'])
+        dpatch = p.gemm_nt(dpatch_t.view(B, P, 3), Rt)                  # x_t = R x: dx = R^T dx_t (rows: dx_t R)
+        dsub = p.gemm_nt(dsub_t.view(B, S, 3), Rt)
+        if self.shared:                                                  # the QSTN saw cat(patch, sub)
+            dsrc = dsrc.view(B, P + S, 3)
+            p.axpy_(dpatch, dsrc[:, :P])
+            p.axpy_(dsub, dsrc[:, P:])
+        else:                                                            # feat_global.stn1 saw the sub-sample
+            p.axpy_(dsub, dsrc)
+        return dpatch, dsub
 
     # ------------------------------------------------------------------------------------------ eval-mode forward
     def evaluate(self, batch):
@@ -470,3 +503,73 @@ class TrainStep:
 
     def named_gradients(self):
         return {name: g.reshape(self._orig_shape[name]) for name, g in self.grads.items()}
+
+
+class EvalGrad(TrainStep):
+    """Gradients of the eval-mode network (`model.eval()`: every BatchNorm uses running_mean / running_var, eps 1e-5)
+    with respect to its parameters and inputs, for autograd through points2surf_b200.model.PointsToSurfModel.
+
+        eg = EvalGrad(state_dict, use_point_stn, shared_transformer, P, S, output_dim=2)
+        eg.forward(batch)                                 # fp32 recompute, records ReLU masks and arg-maxes
+        dpatch, dsub, dquery = eg.backward_inputs(dlogits)   # eg.named_gradients(): every parameter
+
+    TrainStep's network walk and backward run with eval-mode BatchNorm units: the statistics are constants, so the
+    backward is a row-local scaling (p2s_op_bn_eval_backward) and every max-pooled conv3 layer sends its gradient to one
+    point per (query, channel) (p2s_op_bn_maxpool_eval_bwd: weight gradient as a gather over B rows, input gradient as a
+    scatter).  Unlike the train-mode step, the bias in front of a BatchNorm gets its gradient (sum of dz).  Nothing is
+    updated: running statistics and num_batches_tracked stay as they are."""
+
+    _momentum = False
+
+    def __init__(self, state_dict, use_point_stn, shared_transformer, points_per_patch=300, sub_sample_size=1000,
+                 net_size=1024, output_dim=2, device=None, prims=None, dtype=torch.float32):
+        outputs = ('imp_surf',) if output_dim == 1 else ('imp_surf_magnitude', 'imp_surf_sign')
+        super().__init__(state_dict, use_point_stn, shared_transformer, points_per_patch, sub_sample_size, net_size,
+                         device=device, prims=prims, outputs=outputs, dtype=dtype)
+        self._invstd = {k[:-len('.running_var')]: torch.rsqrt(v + BN_EPS) for k, v in self.buffers.items()
+                        if k.endswith('.running_var')}
+
+    def _bn_fwd(self, z, bn, relu):
+        mean, invstd = self.buffers[bn + '.running_mean'], self._invstd[bn]
+        y = self.p.bn_apply(z, mean, invstd, self.params[bn + '.weight'], self.params[bn + '.bias'], relu)
+        return y, mean, invstd
+
+    def _bn_pool_fwd(self, z, bn, relu, B, n):
+        mean, invstd = self.buffers[bn + '.running_mean'], self._invstd[bn]
+        out, arg = self.p.bn_maxpool_apply(z, B, n, mean, invstd, self.params[bn + '.weight'], self.params[bn + '.bias'], relu)
+        return out, arg, mean, invstd
+
+    def _bn_bwd(self, t, dy):
+        p = self.p
+        dz, dgamma, dbeta, dbias = p.bn_eval_backward(dy, t.z, t.y_mask, t.mean, t.invstd, self.params[t.bn + '.weight'])
+        p.axpy_(self.grads[t.bn + '.weight'], dgamma)
+        p.axpy_(self.grads[t.bn + '.bias'], dbeta)
+        p.axpy_(self.grads[t.name + '.bias'], dbias)
+        return dz
+
+    def _lin_bwd(self, t, dy, need_dx=True):
+        if t.pool is None:
+            return super()._lin_bwd(t, dy, need_dx)
+        p = self.p
+        out, arg, B, n = t.pool
+        dx, dgamma, dbeta, dbias = p.bn_maxpool_eval_backward(dy, arg, out, t.z, t.x, self.params[t.name + '.weight'], t.mean,
+                                                              t.invstd, self.params[t.bn + '.weight'], t.relu, B, n,
+                                                              self.grads[t.name + '.weight'], need_dx)
+        p.axpy_(self.grads[t.bn + '.weight'], dgamma)
+        p.axpy_(self.grads[t.bn + '.bias'], dbeta)
+        p.axpy_(self.grads[t.name + '.bias'], dbias)
+        return dx
+
+    def backward_inputs(self, dlogits, dsub_extra=None):
+        """Parameter gradients into self.grads and -> (d patch_pts_ps, d pts_sub_sample_ms, d imp_surf_query_point_ms)
+        through the centring sub = pts_sub_sample_ms - query; dsub_extra [B,S,3]: a gradient that reaches the centred
+        sub-sample by another way (the reference centres the caller's tensor in place, later uses of it add theirs)."""
+        p = self.p
+        dpatch, dsub = self.backward(dlogits, need_inputs=True)
+        if dsub_extra is not None:
+            p.axpy_(dsub, dsub_extra)
+        B = dsub.shape[0]
+        ones = torch.ones((B, self.S, 1), dtype=dsub.dtype, device=dsub.device)
+        dquery = torch.zeros((B, 3), dtype=dsub.dtype, device=dsub.device)
+        p.axpy_(dquery, p.gemm_tn(ones, dsub), -1.0)                     # d query = -sum over the points of d sub
+        return dpatch, dsub, dquery

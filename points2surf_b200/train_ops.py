@@ -135,6 +135,50 @@ class CudaPrims:
                                                  _ptr(s[0]), _ptr(s[1]), _ptr(dz), _stream()))
         return dz, s[1].float(), s[0].float()
 
+    # ---- BatchNorm1d (eval mode: running statistics, mean = running_mean, invstd = rsqrt(running_var + eps))
+    def bn_maxpool_apply(self, z, B, npts, mean, invstd, gamma, beta, relu):
+        """max over the points of act(gamma (z - mean) invstd + beta) with given statistics -> out [B,C], arg [B,C]."""
+        z = _f(z, 'z')
+        Cc = z.shape[1]
+        out = torch.empty((B, Cc), dtype=torch.float32, device=z.device)
+        arg = torch.empty((B, Cc), dtype=torch.int32, device=z.device)
+        with torch.cuda.device(z.device):
+            check(self.lib.p2s_op_bn_maxpool_fwd(_ptr(z), B, npts, Cc, _ptr(_f(mean, 'mean')), _ptr(_f(invstd, 'invstd')),
+                                                 _ptr(_f(gamma, 'gamma')), _ptr(_f(beta, 'beta')), 1 if relu else 0, _ptr(out),
+                                                 _ptr(arg), _stream()))
+        return out, arg
+
+    def bn_eval_backward(self, dy, z, y_mask, mean, invstd, gamma):
+        """-> dz, dgamma, dbeta, dbias (the gradient of the bias in front: sum of dz).  y_mask as in bn_backward."""
+        dy, z = _f(dy, 'dy'), _f(z, 'z')
+        M, Cc = z.shape
+        s = torch.empty((3, Cc), dtype=torch.float64, device=z.device)
+        dz = torch.empty_like(z)
+        with torch.cuda.device(z.device):
+            check(self.lib.p2s_op_bn_eval_backward(_ptr(dy), _ptr(z), _ptr(_f(y_mask, 'y')) if y_mask is not None else None, M, Cc,
+                                                   _ptr(_f(mean, 'mean')), _ptr(_f(invstd, 'invstd')), _ptr(_f(gamma, 'gamma')),
+                                                   _ptr(s[0]), _ptr(s[1]), _ptr(s[2]), _ptr(dz), _stream()))
+        s = s.float()
+        return dz, s[1], s[0], s[2]
+
+    def bn_maxpool_eval_backward(self, dout, arg, out, z, x, W, mean, invstd, gamma, relu, B, npts, dW, need_dx=True):
+        """Backward of conv (x [B*npts, K], W [C, K]) + eval BatchNorm (+ReLU) + max over the points from dout [B, C]:
+        adds the weight gradient into dW [C, K] -> dx [B*npts, K] (None unless need_dx), dgamma, dbeta, dbias."""
+        x, W = _f(x, 'x'), _f(W, 'W')
+        Cc, K = W.shape
+        if not dW.is_contiguous() or dW.dtype != torch.float32 or tuple(dW.shape) != (Cc, K):
+            raise P2SError('bn_maxpool_eval_backward: bad `dW`')
+        s = torch.empty((3, Cc), dtype=torch.float64, device=x.device)
+        dx = torch.empty((B * npts, K), dtype=torch.float32, device=x.device) if need_dx else None
+        with torch.cuda.device(x.device):
+            check(self.lib.p2s_op_bn_maxpool_eval_bwd(_ptr(_f(dout, 'dout')), _ptr(_dev(arg, torch.int32, 'arg')),
+                                                      _ptr(_f(out, 'out')) if relu else None, _ptr(_f(z, 'z')), _ptr(x), _ptr(W),
+                                                      B, npts, Cc, K, _ptr(_f(mean, 'mean')), _ptr(_f(invstd, 'invstd')),
+                                                      _ptr(_f(gamma, 'gamma')), 1 if relu else 0, _ptr(dW), _ptr(s[0]),
+                                                      _ptr(s[1]), _ptr(s[2]), _ptr(dx) if need_dx else None, _stream()))
+        s = s.float()
+        return dx, s[1], s[2], s[0]
+
     def col_sum(self, x):
         x = _f(x, 'x')
         M, Cc = x.shape
