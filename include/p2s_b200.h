@@ -280,6 +280,33 @@ int p2s_mesh_signed_distance_dev(const float* verts, int64_t V, const int32_t* f
 int p2s_mesh_closest_point_dev(const float* verts, int64_t V, const int32_t* faces, int64_t F, const float* query,
                                int64_t Q, float* closest_pts, float* dist, int32_t* closest_face, void* stream);
 
+/* ------------------------------------------------------------------ solid voxelisation --------- */
+/* Inside flag of every voxel centre of a res^3 grid over [-1, 1]^3, 2 <= res <= 1024 (the exact-sign volume of
+ * make_dataset's 06_mc_gt_exact_sign).  Voxel (ix, iy, iz) has the centre (c(ix), c(iy), c(iz)),
+ * c(i) = float(((double)i + 0.5) / res * 2 - 1), the points of p2s_query_points_dev.  It is inside iff the ray from its
+ * centre towards +z crosses an odd number of faces.  The rule is watertight: on a closed mesh (every edge shared by
+ * exactly two faces) every column is crossed an even number of times, whatever the coordinates:
+ *   - x and y are taken in fixed point, X = llrint(double(x) * 2^26), for the vertices and the column centres alike; z
+ *     stays fp32.  Every vertex must have |x| < 16, |y| < 16 and a finite z (else an error), so the edge functions below
+ *     are exact in int64.
+ *   - a column crosses a face iff the face's three projected edge functions E(u -> v) = (u - p) x (v - p), each evaluated
+ *     on the edge's canonical vertex order (lower vertex index first) and negated where the face runs the other way,
+ *     have the same sign.  So the two faces that share an edge see exactly negated values.
+ *   - ties (a column centre on a projected edge or vertex, E == 0) take the sign at the centre moved by (eps, eps^2): the
+ *     sign of -(v.y - u.y), or of v.x - u.x when v.y == u.y (a top-left rule).  Every column thus sees one generic
+ *     point of the projected mesh.
+ *   - faces whose projection has zero area (parallel to z, or with a repeated vertex) cross no column.
+ *   - the crossing height is z = (E_bc z_a + E_ca z_b + E_ab z_c) / (E_bc + E_ca + E_ab) in float64 (each E rounded to
+ *     float64, sums left to right, no contraction); the crossing flips every voxel of the column with c(iz) < z.
+ * The flags are an inside/outside sign only for closed meshes; on other meshes they are the rule's parity.  On a closed
+ * mesh the parity is the winding number mod 2: where closed components overlap (winding number 2) a voxel is outside,
+ * while p2s_mesh_signed_distance_dev's w > 0.5 calls it inside.
+ *   verts [V,3] fp32, faces [F,3] int32 (every index in [0, V), else an error; F = 0 gives all 0)
+ *   inside [res^3] uint8: 1 inside, 0 outside, at (ix * res + iy) * res + iz (the order of p2s_query_grid_dev's indices).
+ * Bitwise deterministic.  sync: input check read-back. */
+int p2s_mesh_inside_grid_dev(const float* verts, int64_t V, const int32_t* faces, int64_t F, int res, uint8_t* inside,
+                             void* stream);
+
 /* ------------------------------------------------------------------ input point clouds --------- */
 /* Simulated time-of-flight range scans: the BlenSor scans of make_dataset.py:sample_blensor (make_dataset.py:242-380,
  * scanner settings blensor_script_template.py:80-96) merged in model space like _pcd_files_to_pts

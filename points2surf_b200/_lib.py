@@ -123,6 +123,7 @@ SIGNATURES = {
     'p2s_chamfer_hausdorff_dev': (C.c_int, [_vp, _i64, _vp, _i64, C.POINTER(C.c_double), _vp]),
     'p2s_mesh_signed_distance_dev': (C.c_int, [_vp, _i64, _vp, _i64, _vp, _i64, _vp, _vp, _vp, _vp]),
     'p2s_mesh_closest_point_dev': (C.c_int, [_vp, _i64, _vp, _i64, _vp, _i64, _vp, _vp, _vp, _vp]),
+    'p2s_mesh_inside_grid_dev': (C.c_int, [_vp, _i64, _vp, _i64, _i32, _vp, _vp]),
     'p2s_range_scan_dev': (C.c_int, [_vp, _i64, _vp, _i64, _vp, _i64, C.POINTER(ScanConfig), C.c_uint64, _vp, _vp, _vp,
                                      _i64, _vp, C.POINTER(_i64), _vp]),
     'p2s_mesh_clean_dev': (C.c_int, [_vp, _i64, _vp, _i64, _vp, _i64, _vp, _i64, C.POINTER(CleanReport), _vp]),

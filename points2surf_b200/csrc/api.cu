@@ -534,6 +534,14 @@ int p2s_mesh_closest_point_dev(const float* verts, int64_t V, const int32_t* fac
     });
 }
 
+int p2s_mesh_inside_grid_dev(const float* verts, int64_t V, const int32_t* faces, int64_t F, int res, uint8_t* inside,
+                             void* stream) {
+    return guarded([&] {
+        P2S_CHECK((verts || V == 0) && (faces || F == 0) && inside, "null argument");
+        mesh_inside_grid(verts, V, faces, F, res, inside, as_stream(stream));
+    });
+}
+
 int p2s_range_scan_dev(const float* verts, int64_t V, const int32_t* faces, int64_t F, const double* poses, int64_t S,
                        const p2s_scan_config* cfg, uint64_t seed, float* pts_noisy, float* pts_clean, int32_t* face_ids,
                        int64_t cap, int32_t* hits_per_scan, int64_t* total_host, void* stream) {

@@ -127,6 +127,9 @@ void mesh_signed_distance(const float* verts, int64_t V, const int32_t* faces, i
                           float* dist, int32_t* closest_face, float* winding, cudaStream_t st);
 void mesh_closest_point(const float* verts, int64_t V, const int32_t* faces, int64_t F, const float* query, int64_t Q,
                         float* closest, float* dist, int32_t* closest_face, cudaStream_t st);
+// inside.cu
+void mesh_inside_grid(const float* verts, int64_t V, const int32_t* faces, int64_t F, int res, uint8_t* inside,
+                      cudaStream_t st);
 // scan.cu
 void range_scan(const float* verts, int64_t V, const int32_t* faces, int64_t F, const double* poses, int64_t S,
                 const p2s_scan_config& cfg, uint64_t seed, float* pts_noisy, float* pts_clean, int32_t* face_ids,

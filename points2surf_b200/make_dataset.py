@@ -5,10 +5,15 @@
     (csrc/scan.cu) instead of Blender / BlenSor, with the reference's scan poses and noise levels;
   - the training targets 05_query_pts / 05_query_dist (and optionally 05_query_vis) of the query-point stage
     (make_dataset.py:447-538), with the signed distances of csrc/meshsdf.cu;
-  - clean_up_broken_inputs, make_dataset_splits and make_dataset, which runs all of it (--from_base_meshes).
+  - clean_up_broken_inputs, make_dataset_splits and make_dataset, which runs all of it (--from_base_meshes);
+  - with --gt_recon, reconstruct_gt (make_dataset.py:649-712) in model space: the grid targets 05_query_pts_grid /
+    05_query_dist_grid, meshes from them through sign propagation (06_mc_gt_recon) and with the exact inside/outside sign
+    of every voxel (06_mc_gt_exact_sign, csrc/inside.cu), and their Chamfer reports.
 
     python -m points2surf_b200.make_dataset DATASET_DIR [--scan] [--num_query_pts 2000] [--far_query_pts_ratio 0.5] [--debug]
     python -m points2surf_b200.make_dataset DATASET_DIR --from_base_meshes [--num_query_pts 2000]
+    python -m points2surf_b200.make_dataset DATASET_DIR --gt_recon [--grid_resolution 256] [--epsilon 3] [--sigma 5]
+                                                                 [--certainty_threshold 13] [--dataset testset.txt]
 
 From DATASET_DIR/settings.ini: patch_radius = (1 + epsilon) / grid_resolution (make_dataset.py:760); with --scan also
 num_scans_per_mesh_min/max, scanner_noise_sigma_min/max and only_for_evaluation (make_dataset.py:809-815)."""
@@ -23,6 +28,7 @@ import sys
 import numpy as np
 import torch
 
+from . import evaluation
 from . import mesh_io
 from . import ops
 from . import sdf
@@ -38,6 +44,15 @@ def filename_to_hash(file_path):
     return int(hashlib.md5(stem.encode()).hexdigest(), 16) % (2 ** 32 - 1)
 
 
+def _signed_distance_target(mesh, query_pts_ms, signed_distance_batch_size=1000):
+    """The signed-distance target of make_dataset.py:464-474: sdf.get_signed_distance with NaN -> 0, Inf -> 1, clamped to
+    [-1, 1] (float64; the files store it as float32)."""
+    query_dist_ms = sdf.get_signed_distance(mesh, query_pts_ms, signed_distance_batch_size)
+    query_dist_ms[np.isnan(query_dist_ms)] = 0.0
+    query_dist_ms[np.isinf(query_dist_ms)] = 1.0
+    return np.clip(query_dist_ms, -1.0, 1.0)
+
+
 def _get_and_save_query_pts(file_in_mesh, file_out_query_pts, file_out_query_dist, file_out_query_vis, num_query_pts,
                             patch_radius, far_query_pts_ratio=0.1, signed_distance_batch_size=1000, debug=False):
     """make_dataset.py:447-478 for one mesh: float32 query points and distances (NaN -> 0, Inf -> 1, clamped to [-1, 1])."""
@@ -45,10 +60,7 @@ def _get_and_save_query_pts(file_in_mesh, file_out_query_pts, file_out_query_dis
     mesh = mesh_io.read_ply(file_in_mesh)
     query_pts_ms = sdf.get_query_pts_for_mesh(mesh, num_query_pts, patch_radius, far_query_pts_ratio, rng)
     np.save(file_out_query_pts, query_pts_ms.astype(np.float32))
-    query_dist_ms = sdf.get_signed_distance(mesh, query_pts_ms, signed_distance_batch_size)
-    query_dist_ms[np.isnan(query_dist_ms)] = 0.0
-    query_dist_ms[np.isinf(query_dist_ms)] = 1.0
-    query_dist_ms = np.clip(query_dist_ms, -1.0, 1.0)
+    query_dist_ms = _signed_distance_target(mesh, query_pts_ms, signed_distance_batch_size)
     np.save(file_out_query_dist, query_dist_ms.astype(np.float32))
     if debug and file_out_query_vis is not None:
         sdf.visualize_query_points(query_pts_ms, query_dist_ms, file_out_query_vis)
@@ -78,6 +90,138 @@ def get_query_pts_dist_ms(base_dir, dataset_dir, dir_in_mesh, dir_out_query_pts_
         if sdf._call_necessary([file_in_mesh], [file_out_query_pts, file_out_query_dist]):
             _get_and_save_query_pts(file_in_mesh, file_out_query_pts, file_out_query_dist, file_out_query_vis,
                                     num_query_pts, patch_radius, far_query_pts_ratio, signed_distance_batch_size, debug)
+
+
+def get_query_pts_dist_grid(base_dir, dataset_dir, dir_in_pts, dir_in_mesh, dir_out_query_pts, dir_out_query_dist,
+                            grid_resolution, epsilon):
+    """The grid targets that the reference's reconstruct_gt reads, in model space: for every <name>.xyz.npy in dir_in_pts
+    with a dir_in_mesh/<name>.ply whose outputs are missing or older than either input,
+      dir_out_query_pts/<name>.xyz.npy  float32 [Q, 3] = sdf.get_voxel_centers_grid_smaller_pc(points, grid_resolution,
+                                        epsilon), the query points of the reconstruction at that resolution and epsilon;
+      dir_out_query_dist/<name>.xyz.npy float32 [Q] = the mesh's signed distances there, cleaned up like 05_query_dist.
+    Columns 0:3 of the point cloud are the points.  No 05_patch_ids_grid: model-space points need no patch centre."""
+    root = os.path.join(base_dir, dataset_dir)
+    dir_pts, dir_mesh = os.path.join(root, dir_in_pts), os.path.join(root, dir_in_mesh)
+    dir_q, dir_d = os.path.join(root, dir_out_query_pts), os.path.join(root, dir_out_query_dist)
+    os.makedirs(dir_q, exist_ok=True)
+    os.makedirs(dir_d, exist_ok=True)
+    for f in sorted(f for f in os.listdir(dir_pts) if os.path.isfile(os.path.join(dir_pts, f)) and f[-8:] == '.xyz.npy'):
+        file_pts, file_mesh = os.path.join(dir_pts, f), os.path.join(dir_mesh, f[:-8] + '.ply')
+        file_q, file_d = os.path.join(dir_q, f), os.path.join(dir_d, f)
+        if not os.path.isfile(file_mesh) or not sdf._call_necessary([file_pts, file_mesh], [file_q, file_d]):
+            continue
+        query_pts_ms = sdf.get_voxel_centers_grid_smaller_pc(np.load(file_pts)[:, :3], grid_resolution, epsilon)
+        np.save(file_q, query_pts_ms.astype(np.float32))
+        query_dist_ms = _signed_distance_target(mesh_io.read_ply(file_mesh), query_pts_ms)
+        np.save(file_d, query_dist_ms.astype(np.float32))
+
+
+def reconstruct_gt(base_dir, dataset_dir, pts_dir, query_dist_dir, query_pts_dir, gt_reconstruction_dir,
+                   grid_resolution, sigma, certainty_threshold, num_processes=1):
+    """make_dataset.py:662-712, the reconstruction from ground-truth signed distances, on model-space grid files (the
+    reference's patch-space call cannot run: it omits patch_space_to_model_space's patch radius), so the signature has no
+    p_ids_grid_dir.  For every <name>.xyz.npy in query_dist_dir whose outputs are missing or older than an input:
+    sdf.implicit_surface_to_mesh -> gt_reconstruction_dir/<name>.ply and gt_reconstruction_dir/vol/<name>.xyz.off.
+    `num_processes` is accepted and ignored."""
+    root = os.path.join(base_dir, dataset_dir)
+    dir_mesh = os.path.join(root, gt_reconstruction_dir)
+    dir_vol = os.path.join(dir_mesh, 'vol')
+    os.makedirs(dir_vol, exist_ok=True)
+    dir_d = os.path.join(root, query_dist_dir)
+    for f in sorted(f for f in os.listdir(dir_d) if os.path.isfile(os.path.join(dir_d, f)) and f[-8:] == '.xyz.npy'):
+        file_pts, file_d, file_q = (os.path.join(root, d, f) for d in (pts_dir, query_dist_dir, query_pts_dir))
+        file_vol, file_rec = os.path.join(dir_vol, f[:-4] + '.off'), os.path.join(dir_mesh, f[:-8] + '.ply')
+        if sdf._call_necessary([file_pts, file_d, file_q], [file_rec, file_vol]):
+            sdf.implicit_surface_to_mesh_file(file_d, file_q, file_vol, file_rec, grid_resolution, sigma,
+                                              certainty_threshold)
+
+
+def mesh_is_closed(faces):
+    """True iff every edge is shared by exactly two faces that run it in opposite directions (the condition under which
+    the parity of ops.mesh_inside_grid is an inside/outside sign)."""
+    f = np.asarray(faces, np.int64).reshape(-1, 3)
+    if len(f) == 0:
+        return False
+    e = np.concatenate([f[:, [0, 1]], f[:, [1, 2]], f[:, [2, 0]]])
+    if (e[:, 0] == e[:, 1]).any():
+        return False
+    n = int(e.max()) + 1
+    fwd, cnt = np.unique(e[:, 0] * n + e[:, 1], return_counts=True)
+    # each directed edge once (not in two faces the same way, not in three or more faces) and its reverse present
+    return bool((cnt == 1).all() and np.isin(e[:, 1] * n + e[:, 0], fwd).all())
+
+
+def exact_sign_volume(inside, lin_idx, dist):
+    """The volume [res, res, res] fp32 of the exact-sign reconstruction: the signed distances dist at the voxels lin_idx,
+    clamped to [-1, 1] like ops.sdf_to_volume, and +1 inside / -1 outside (inside [res, res, res] bool) everywhere else."""
+    vol = torch.where(inside, 1.0, -1.0)
+    vol.view(-1)[lin_idx.long()] = dist.clamp(-1.0, 1.0)
+    return vol
+
+
+def reconstruct_gt_exact_sign(base_dir, dataset_dir, mesh_dir, query_dist_dir, query_pts_dir, out_dir, grid_resolution,
+                              sigma, certainty_threshold):
+    """Marching cubes on exact_sign_volume for every <name>.xyz.npy in query_dist_dir with a closed mesh_dir/<name>.ply
+    whose output out_dir/<name>.ply is missing or older than an input; the inside flags come from ops.mesh_inside_grid.
+    Prints per shape Q and the number of voxels whose sign after sign propagation (ops.sdf_to_volume on the same distances
+    with sigma and certainty_threshold; a voxel left at 0 counts as outside) differs from the exact sign.  A mesh that is
+    not closed gets one line and no output."""
+    root = os.path.join(base_dir, dataset_dir)
+    dir_out = os.path.join(root, out_dir)
+    os.makedirs(dir_out, exist_ok=True)
+    dir_d = os.path.join(root, query_dist_dir)
+    dev = sdf._device()
+    for f in sorted(f for f in os.listdir(dir_d) if os.path.isfile(os.path.join(dir_d, f)) and f[-8:] == '.xyz.npy'):
+        name = f[:-8]
+        file_mesh = os.path.join(root, mesh_dir, name + '.ply')
+        file_d, file_q = os.path.join(dir_d, f), os.path.join(root, query_pts_dir, f)
+        file_rec = os.path.join(dir_out, name + '.ply')
+        if not os.path.isfile(file_mesh) or not sdf._call_necessary([file_mesh, file_d, file_q], [file_rec]):
+            continue
+        verts, faces = mesh_io.read_ply(file_mesh)
+        if not mesh_is_closed(faces):
+            print('{}: mesh is not closed (an edge not shared by exactly two opposite faces), no exact-sign '
+                  'reconstruction'.format(name))
+            continue
+        inside = ops.mesh_inside_grid(torch.from_numpy(np.ascontiguousarray(verts, np.float32)).to(dev),
+                                      torch.from_numpy(np.ascontiguousarray(faces, np.int32)).to(dev), grid_resolution)
+        lin = sdf.volume_lin_idx(np.load(file_q), grid_resolution)
+        dist = torch.from_numpy(np.ascontiguousarray(np.load(file_d), np.float32)).to(dev)
+        vol = exact_sign_volume(inside, lin, dist)
+        prop, _ = ops.sdf_to_volume(lin, dist, grid_resolution, sigma, certainty_threshold)
+        print('{}: {} grid queries, {} voxels with a propagated sign other than the exact sign'.format(
+            name, len(dist), int(((prop > 0.0) != (vol > 0.0)).sum())))
+        v, fc = ops.marching_cubes(vol, 0.0)
+        if len(fc) == 0:
+            print('Warning: marching cubes gives no result for {}'.format(name))
+            continue
+        mesh_io.write_ply(file_rec, v.cpu().numpy(), fc.cpu().numpy())
+
+
+def gt_recon(dataset, grid_resolution=256, epsilon=3, sigma=5, certainty_threshold=13, dataset_file='testset.txt'):
+    """Where the reconstruction error comes from: 05_query_pts_grid / 05_query_dist_grid, then meshes from the
+    ground-truth distances through sign propagation (06_mc_gt_recon) and with every voxel's exact sign
+    (06_mc_gt_exact_sign), then their Hausdorff / Chamfer reports against 03_meshes for the shapes in dataset_file
+    (comp_mc_gt_recon.csv, comp_mc_gt_exact_sign.csv)."""
+    base_dir, dataset_dir = os.path.dirname(dataset), os.path.basename(dataset)
+    print('### grid query points, signed distances')
+    get_query_pts_dist_grid(base_dir, dataset_dir, '04_pts', '03_meshes', '05_query_pts_grid', '05_query_dist_grid',
+                            grid_resolution, epsilon)
+    print('### reconstruct from ground-truth signed distances')
+    reconstruct_gt(base_dir, dataset_dir, '04_pts', '05_query_dist_grid', '05_query_pts_grid', '06_mc_gt_recon',
+                   grid_resolution, sigma, certainty_threshold)
+    print('### reconstruct from ground-truth signed distances with exact signs')
+    reconstruct_gt_exact_sign(base_dir, dataset_dir, '03_meshes', '05_query_dist_grid', '05_query_pts_grid',
+                              '06_mc_gt_exact_sign', grid_resolution, sigma, certainty_threshold)
+    for rec_dir, report in (('06_mc_gt_recon', 'comp_mc_gt_recon.csv'), ('06_mc_gt_exact_sign', 'comp_mc_gt_exact_sign.csv')):
+        rec_dir_abs = os.path.join(dataset, rec_dir)
+        if not any(f[-4:] == '.ply' for f in os.listdir(rec_dir_abs)):
+            print('### {}: no meshes to compare'.format(rec_dir))
+            continue
+        print('### {} - hausdorff distance'.format(rec_dir))
+        evaluation.mesh_comparison(new_meshes_dir_abs=rec_dir_abs, ref_meshes_dir_abs=os.path.join(dataset, '03_meshes'),
+                                   num_processes=1, report_name=os.path.join(dataset, report), samples_per_model=10000,
+                                   dataset_file_abs=os.path.join(dataset, dataset_file))
 
 
 def get_scan_poses(file_in_mesh, num_scans_per_mesh_min, num_scans_per_mesh_max, scanner_noise_sigma_min=0.0,
@@ -393,8 +537,22 @@ def main(argv=None):
     parser.add_argument('--from_base_meshes', action='store_true',
                         help='run the whole make_dataset from DATASET_DIR/00_base_meshes (convert, clean, normalise, '
                              'scan, query points, splits); --scan, --debug and --far_query_pts_ratio do not apply')
+    parser.add_argument('--gt_recon', action='store_true',
+                        help='instead of the query stage, reconstruct from ground-truth signed distances on the '
+                             'reconstruction grid of 04_pts: 05_query_pts_grid, 05_query_dist_grid, 06_mc_gt_recon (sign '
+                             'propagation), 06_mc_gt_exact_sign (exact signs, closed meshes only) and their reports '
+                             'comp_mc_gt_recon.csv, comp_mc_gt_exact_sign.csv')
+    parser.add_argument('--grid_resolution', type=int, default=256, help='--gt_recon: the reconstruction grid resolution')
+    parser.add_argument('--epsilon', type=int, default=3,
+                        help='--gt_recon: voxels around the points that get a query (not settings.ini\'s epsilon)')
+    parser.add_argument('--sigma', type=int, default=5, help='--gt_recon: sign propagation window')
+    parser.add_argument('--certainty_threshold', type=float, default=13, help='--gt_recon: sign propagation threshold')
+    parser.add_argument('--dataset', default='testset.txt', help='--gt_recon: the shapes to compare with 03_meshes')
     args = parser.parse_args(argv)
     dataset = os.path.abspath(args.dataset_dir)
+    if args.gt_recon:
+        gt_recon(dataset, args.grid_resolution, args.epsilon, args.sigma, args.certainty_threshold, args.dataset)
+        return
     if args.from_base_meshes:
         make_dataset(os.path.basename(dataset), None, os.path.dirname(dataset),
                      num_query_points_per_shape=args.num_query_pts)

@@ -345,6 +345,24 @@ def mesh_closest_point(verts, faces, query):
     return closest, dist, fid
 
 
+def mesh_inside_grid(verts, faces, res):
+    """Inside flag [res, res, res] bool of every voxel centre ((i + 0.5) / res) * 2 - 1 of [-1, 1]^3, indexed [ix, iy, iz]:
+    the parity of the faces the ray from the centre towards +z crosses, by the watertight rule of include/p2s_b200.h
+    ("solid voxelisation").  An inside/outside sign only for closed meshes.  Vertices need |x|, |y| < 16."""
+    verts = _dev(verts, torch.float32, 'verts')
+    faces = _dev(faces, torch.int32, 'faces')
+    if verts.dim() != 2 or verts.shape[1] != 3 or faces.dim() != 2 or faces.shape[1] != 3:
+        raise P2SError('verts and faces must have shape [n, 3]')
+    res = int(res)
+    if not 2 <= res <= 1024:
+        raise P2SError('grid resolution out of range')
+    inside = torch.empty((res, res, res), dtype=torch.bool, device=verts.device)
+    with torch.cuda.device(verts.device):
+        check(_lib.load().p2s_mesh_inside_grid_dev(_ptr(verts), verts.shape[0], _ptr(faces), faces.shape[0], res,
+                                                   _ptr(inside), _stream()))
+    return inside
+
+
 def mesh_clean(verts, faces):
     """The mesh repair of make_dataset.py:_clean_mesh (rules and output order in include/p2s_b200.h): weld, drop
     non-finite, degenerate and duplicate faces, fill 3- and 4-edge holes, orient every component consistently and

@@ -28,6 +28,17 @@ def model_space_to_volume_space(pts_ms, vol_res):
     return np.floor(((pts_ms + 1.0) / 2.0) * vol_res).astype(int)
 
 
+def volume_lin_idx(query_pts_ms, grid_res):
+    """The voxels of the query points (model_space_to_volume_space) as int32 linear indices (ix * res + iy) * res + iz on
+    the device, the scatter order of ops.sdf_to_volume."""
+    idx = model_space_to_volume_space(np.asarray(query_pts_ms), grid_res)
+    if idx.size and (idx.min() < 0 or idx.max() >= grid_res):
+        # the reference raises IndexError for an index >= grid_res and silently wraps a negative one
+        # (sdf.py:95-111, SURVEY section 10 "Precondition"); both are rejected here, nothing is written out of bounds
+        raise IndexError('query points outside [-1, 1)^3: voxel index out of range for grid resolution %d' % grid_res)
+    return torch.from_numpy(((idx[:, 0] * grid_res + idx[:, 1]) * grid_res + idx[:, 2]).astype(np.int32)).to(_device())
+
+
 def implicit_surface_to_mesh(query_dist_ms, query_pts_ms, volume_out_file, mc_out_file, grid_res, sigma,
                              certainty_threshold=26):
     """source/sdf.py:181-230: scatter -> sign propagation -> clamp -> marching cubes -> PLY.
@@ -37,12 +48,7 @@ def implicit_surface_to_mesh(query_dist_ms, query_pts_ms, volume_out_file, mc_ou
         print('WARNING: implicit surface for {} contains only zeros'.format(volume_out_file))
         return
     dev = _device()
-    idx = model_space_to_volume_space(np.asarray(query_pts_ms), grid_res)
-    if idx.size and (idx.min() < 0 or idx.max() >= grid_res):
-        # the reference raises IndexError for an index >= grid_res and silently wraps a negative one
-        # (sdf.py:95-111, SURVEY section 10 "Precondition"); both are rejected here, nothing is written out of bounds
-        raise IndexError('query points outside [-1, 1)^3: voxel index out of range for grid resolution %d' % grid_res)
-    lin = torch.from_numpy(((idx[:, 0] * grid_res + idx[:, 1]) * grid_res + idx[:, 2]).astype(np.int32)).to(dev)
+    lin = volume_lin_idx(query_pts_ms, grid_res)
     sdf = torch.from_numpy(np.ascontiguousarray(query_dist_ms, dtype=np.float32)).to(dev)
     start = time.time()
     vol, _ = ops.sdf_to_volume(lin, sdf, grid_res, sigma, certainty_threshold)
