@@ -68,9 +68,13 @@ __device__ __forceinline__ void st_async_v4(uint32_t addr, const uint32_t (&v)[4
     asm volatile("st.async.shared::cluster.mbarrier::complete_tx::bytes.v4.b32 [%0], {%1, %2, %3, %4}, [%5];"
                  ::"r"(addr), "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(bar_addr) : "memory");
 }
-// arrive on an mbarrier of any CTA of the cluster (shared::cluster address), releasing this thread's prior accesses
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t bar_addr) {
-    asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(bar_addr) : "memory");
+// arrive on an mbarrier of any CTA of the cluster (shared::cluster address) with the default semantics, release at CTA
+// scope: unlike .release.cluster it compiles to no GPU-scope fence, and it publishes none of this thread's prior writes
+// to the other CTA -- for handing back a buffer this thread only read.  Predicated on `arrive` inside the instruction, so a
+// caller in the middle of an unrolled MMA pipeline needs no branch (one costs the pass kernel its spill-free allocation)
+__device__ __forceinline__ void mbar_arrive_cluster(uint32_t bar_addr, bool arrive) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %1, 0;\n\t@p mbarrier.arrive.shared::cluster.b64 _, [%0];\n\t}"
+                 ::"r"(bar_addr), "r"((uint32_t)arrive) : "memory");
 }
 // wait on a local mbarrier whose arrivals come from other CTAs of the cluster: acquires what they released
 __device__ __forceinline__ bool mbar_try_wait_cluster(uint64_t* bar, uint32_t parity) {
@@ -104,6 +108,14 @@ __device__ __forceinline__ void bulk_g2s(void* smem_dst, const void* gmem_src, u
     asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
                  ::"r"(smem_u32(smem_dst)), "l"(gmem_src), "r"(bytes), "r"(smem_u32(bar)) : "memory");
 }
+
+// ---------------------------------------------------------------- asynchronous copy (cp.async, per thread)
+// 4-byte global -> shared copy; completes at the thread's next cp_async_wait_all after a cp_async_commit
+__device__ __forceinline__ void cp_async_4(void* smem_dst, const void* gmem_src) {
+    asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(smem_u32(smem_dst)), "l"(gmem_src) : "memory");
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+__device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_group 0;" ::: "memory"); }
 
 // ---------------------------------------------------------------- descriptors
 // Shared-memory matrix descriptor, no swizzle ("interleave"), K-major operand of 16-bit elements:
