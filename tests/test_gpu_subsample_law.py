@@ -1,16 +1,11 @@
 """Every sub-sample kernel against the exact law of the reference's draw.
 
-Weighted: each case of tests/subsample_cases.py runs on every kernel it reaches (cells, rejection, cached and uncached
-clocks); the inclusion counts are tested per point against Binomial(T, pi_i) and per distance bin by batch means, with pi
-from oracle/subsample_law.py, and the tiny clouds by Pearson chi-square over all sets.  The kernel switches are read once
-per process, so each environment runs in a subprocess that writes its counts.
+Weighted: the cases of tests/subsample_cases.py put every geometry class on each of the three kernels (cells, cached and
+uncached clocks), which the cloud size selects; the inclusion counts are tested per point against Binomial(T, pi_i) and per
+distance bin by batch means, with pi from oracle/subsample_law.py, and the tiny clouds by Pearson chi-square over all sets.
 Uniform: chi-square on ids and on pairs of adjacent slots inside and across Philox quads.
 Ball query: inclusion k / count for every point of the ball and pairwise inclusion k (k-1) / (count (count-1)) on pairs of
 ids that share a Philox quad, on each branch (count <= k, k < count <= 2048, count > 2048)."""
-import os
-import subprocess
-import sys
-
 import numpy as np
 import pytest
 import torch
@@ -24,64 +19,36 @@ import subsample_cases as sc
 pytestmark = pytest.mark.gpu
 DEV = 'cuda:0'
 SEED = 20261016
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-_WORKER = r"""
-import sys, numpy as np, torch
-sys.path.insert(0, %(root)r); sys.path.insert(0, %(root)r + '/tests')
-from points2surf_b200 import ops
-import subsample_cases as sc
-cases = sc.cases()
-out = {}
-for name in sys.argv[2:]:
-    c = cases[name]
-    cloud = torch.from_numpy(c['cloud']).cuda()
-    N, S, T = len(c['cloud']), c['S'], c['T']
-    per = T // sc.BATCHES
-    q = torch.from_numpy(np.ascontiguousarray(np.repeat(c['query'][None], per, axis=0))).cuda()
-    counts = torch.zeros((sc.BATCHES, N), dtype=torch.int64, device='cuda')
-    sets = torch.zeros(1 << N if N <= 16 else 1, dtype=torch.int64, device='cuda')
-    dup = 0
-    for b in range(sc.BATCHES):
-        ids = ops.subsample(cloud, q, S, False, %(seed)d, query_index_base=b * per).long()
-        counts[b] = torch.bincount(ids.view(-1), minlength=N)
-        s = torch.sort(ids, dim=1).values
-        dup += int((s[:, 1:] == s[:, :-1]).sum()) + int(((s < 0) | (s >= N)).sum())
-        if N <= 16:
-            sets += torch.bincount((1 << ids).sum(1), minlength=1 << N)
-    out[name + '/counts'] = counts.cpu().numpy()
-    out[name + '/sets'] = sets.cpu().numpy()
-    out[name + '/dup'] = np.array(dup)
-np.savez(sys.argv[1], **out)
-"""
 
 
 @pytest.fixture(scope='module')
-def law_counts(tmp_path_factory):
-    d = tmp_path_factory.mktemp('law')
+def law_counts():
     res = {}
-    for env, extra in sc.ENVS.items():
-        names = [n for n, e in sc.runs() if e == env]
-        if not names:
-            continue
-        path = str(d / (env + '.npz'))
-        e = dict(os.environ)
-        e.update(extra)
-        r = subprocess.run([sys.executable, '-c', _WORKER % dict(root=ROOT, seed=SEED), path] + names, env=e,
-                           capture_output=True, text=True, timeout=900)
-        assert r.returncode == 0, (env, r.stdout[-2000:], r.stderr[-3000:])
-        z = np.load(path)
-        for n in names:
-            res[(n, env)] = {k: z[n + '/' + k] for k in ('counts', 'sets', 'dup')}
+    for name, c in sc.cases().items():
+        cloud = torch.from_numpy(c['cloud']).to(DEV)
+        N, S, T = len(c['cloud']), c['S'], c['T']
+        per = T // sc.BATCHES
+        q = torch.from_numpy(np.ascontiguousarray(np.repeat(c['query'][None], per, axis=0))).to(DEV)
+        counts = torch.zeros((sc.BATCHES, N), dtype=torch.int64, device=DEV)
+        sets = torch.zeros(1 << N if N <= 16 else 1, dtype=torch.int64, device=DEV)
+        dup = 0
+        for b in range(sc.BATCHES):
+            ids = ops.subsample(cloud, q, S, False, SEED, query_index_base=b * per).long()
+            counts[b] = torch.bincount(ids.view(-1), minlength=N)
+            s = torch.sort(ids, dim=1).values
+            dup += int((s[:, 1:] == s[:, :-1]).sum()) + int(((s < 0) | (s >= N)).sum())
+            if N <= 16:
+                sets += torch.bincount((1 << ids).sum(1), minlength=1 << N)
+        res[name] = dict(counts=counts.cpu().numpy(), sets=sets.cpu().numpy(), dup=dup)
     return res
 
 
-@pytest.mark.parametrize('name,env', sc.runs())
-def test_weighted_kernel_realises_the_law(law_counts, name, env):
+@pytest.mark.parametrize('name', sc.runs())
+def test_weighted_kernel_realises_the_law(law_counts, name):
     c = sc.cases()[name]
     cloud, q, S, T = c['cloud'], c['query'], c['S'], c['T']
     N = len(cloud)
-    got = law_counts[(name, env)]
+    got = law_counts[name]
     assert int(got['dup']) == 0                                  # S distinct ids in range in every trial
     w = law.weights(cloud, q)
     pi = law.inclusion_probabilities(w, S, device=DEV)
@@ -90,10 +57,9 @@ def test_weighted_kernel_realises_the_law(law_counts, name, env):
     bins = law.equal_mass_bins(pi, np.linalg.norm(cloud.astype(np.float64) - q.astype(np.float64), axis=1))
     t = sc.binned_t(got['counts'], T, pi, bins)
     tmax = float(np.nanmax(np.abs(np.where(np.isfinite(t), t, 0.0))))
-    print('%s [%s, %s]: T=%d max|z|=%.2f max|t|=%.2f (bound %.2f)' % (name, sc.kernel_for(N, S, env), env, T, zmax, tmax,
-                                                                        sc.t_bound()))
-    assert p > sc.ALPHA, (name, env, zmax, p)
-    assert tmax < sc.t_bound(), (name, env, t)
+    print('%s [%s]: T=%d max|z|=%.2f max|t|=%.2f (bound %.2f)' % (name, sc.kernel_for(N, S), T, zmax, tmax, sc.t_bound()))
+    assert p > sc.ALPHA, (name, zmax, p)
+    assert tmax < sc.t_bound(), (name, t)
     if N <= 16:
         full = law.set_law(w, S)
         keys = [sum(1 << i for i in s) for s in full]

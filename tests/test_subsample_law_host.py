@@ -7,6 +7,8 @@ from oracle import p2s_oracle as orc
 from oracle import subsample_law as law
 import subsample_cases as sc
 
+TINY = [n for n in sc.runs() if n.startswith('tiny_')]
+
 
 @pytest.mark.parametrize('N,S', [(5, 2), (8, 3), (8, 5), (9, 1), (9, 4), (9, 8)])
 def test_integral_matches_enumeration(N, S):
@@ -18,7 +20,7 @@ def test_integral_matches_enumeration(N, S):
 
 
 def test_tiny_cases_match_enumeration():
-    for name in ('tiny_8_3', 'tiny_8_5'):
+    for name in TINY:
         c = sc.cases()[name]
         w = law.weights(c['cloud'], c['query'])
         exact = law.set_inclusion(law.set_law(w, c['S']), len(w))
@@ -82,7 +84,7 @@ def test_agrees_with_randomstate_choice():
 
 
 def test_tiny_cases_expect_every_set_five_times():
-    for name in ('tiny_8_3', 'tiny_8_5'):
+    for name in TINY:
         c = sc.cases()[name]
         probs = np.array(list(law.set_law(law.weights(c['cloud'], c['query']), c['S']).values()))
         assert probs.min() * c['T'] >= 5, (name, probs.min() * c['T'])
