@@ -255,7 +255,11 @@ int p2s_chamfer_hausdorff_dev(const float* a, int64_t na, const float* b, int64_
 /* trimesh.proximity.signed_distance as called by sdf.get_signed_distance (source/sdf.py:318-348) for the query points
  * of make_dataset.py:_get_and_save_query_pts (make_dataset.py:447-478).  Exhaustive and exact: the distance to the
  * nearest triangle is the float64 minimum (an fp32 pass selects the faces to recompute within a stated error bound;
- * ties -> lowest face index); zero-area faces count as segments / points.  Sign from the generalised winding number w
+ * ties -> lowest face index); zero-area faces count as segments / points.  Any finite coordinates: the fp32 pass runs
+ * in units of a power of two taken from max(|query|_inf, max |vertex coordinate|), so it neither under- nor overflows,
+ * and the float64 recompute covers fp32's whole range.  So scaling the mesh and the queries by 2^k scales the distance
+ * and the closest point by 2^k bit for bit and keeps the face and the winding number, wherever the scaled inputs and
+ * results are normal fp32 numbers (the sign follows the absolute |d| <= 1e-8 rule below).  Sign from the generalised winding number w
  * (float64 solid angles of all faces): dist = +|d| if w > 0.5 or |d| <= 1e-8 (points on the surface are positive, like
  * trimesh), else -|d|; inside is positive.  w equals trimesh's ray-parity inside test on closed, consistently oriented
  * meshes; on meshes with holes or flipped faces the two can disagree.  A query with a non-finite coordinate gives NaN.

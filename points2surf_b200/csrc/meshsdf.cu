@@ -5,9 +5,10 @@
 //      (the scale of the fp32 error bound below)
 //   2. meshsdf_slab_kernel: grid (query blocks, face slabs); every CTA stages tiles of its slab's triangles in shared
 //      memory, one query per thread, faces in ascending order.  Per face:
-//        - squared distance in fp32; every face whose fp32 value lies within kRelTol / the eps(scale) bound of the
-//          running fp32 minimum is recomputed in float64 and the float64 minimum kept (strict <: lowest face on ties).
-//          Degenerate and sliver faces (|n|^2 < 2^-10 * longest edge^4) skip the fp32 value and always go to float64.
+//        - squared distance in fp32, in units of the query's power-of-two scale; every face whose fp32 value lies
+//          within kRelTol / the eps(scale) bound of the running fp32 minimum is recomputed in float64 and the float64
+//          minimum kept (strict <: lowest face on ties).  Degenerate and sliver faces (|n|^2 < 2^-10 * longest edge^4)
+//          skip the fp32 value and always go to float64, and so do faces too small for fp32 at that scale.
 //        - float64 solid angle (Van Oosterom & Strackee 1983) summed into the slab's winding-number partial; zero-area
 //          faces contribute 0.
 //      -> per (slab, query): float64 d^2, face, float64 winding partial.  Slab boundaries depend on F only.
@@ -41,8 +42,16 @@ constexpr int64_t kChunk = 1 << 18;   // queries per launch pair (bounds the per
 // 2^-10 * d^2 + 2 d eps + eps^2 with eps = 2^-12 * (|p|_inf + max |vertex coordinate|): the coordinate differences
 // carry u * scale, the normal direction 2^5 u, and the rest is a handful of roundings.  The face with the exact minimum
 // therefore always passes `d2f <= best32 + tol(best32)` (tol covers the error on both sides).
+// The argument needs every fp32 value to be a normal number: |n|^2 ~ l^4 and h^2 ~ l^4 d^2 leave fp32's range for
+// coordinates beyond ~2^31 or below ~2^-31.  So the fp32 pass runs in units of 2^e, the power of two with
+// max(|p|_inf, max |vertex coordinate|) in [2^(e-1), 2^e) (e clamped to [-126, 126]): every operand is then at most 1
+// in magnitude (4 beyond 2^126), no value
+// overflows, and the arithmetic is the unit-scale one bit for bit (scaling by a power of two is exact).  A face whose
+// fp32 |n|^2 falls below kMinNN in those units (an edge below ~2^-22 of the scale) goes to float64, so underflow never
+// moves an fp32 value by more than 2^-50, far inside eps^2 >= 2^-26.
 constexpr float kRelTol = 1.0f / 1024.0f;
 constexpr float kEpsScale = 1.0f / 4096.0f;
+constexpr float kMinNN = 0x1p-100f;
 
 enum : unsigned char { kZeroArea = 1, kForce64 = 2 };
 
@@ -63,15 +72,16 @@ __device__ __forceinline__ T seg_dist2(T px, T py, T pz, T ax, T ay, T az, T bx,
 // squared distance from p to the triangle (a, b, c): the plane distance when p projects inside the triangle, else the
 // nearest edge.  A zero-area face is its three edges (a segment or a point).  When cp is not null, the point that gives
 // this distance goes to cp: the projection onto the plane, or the closest point of the first nearest edge in the order
-// ab, bc, ca.  With cp null the arithmetic is exactly the distance-only one.
+// ab, bc, ca.  With cp null the arithmetic is exactly the distance-only one.  |n|^2 goes to nn_out when it is not null.
 template <class T>
 __device__ __forceinline__ T tri_dist2(T px, T py, T pz, T ax, T ay, T az, T bx, T by, T bz, T cx, T cy, T cz,
-                                       bool zero_area, T* cp = nullptr) {
+                                       bool zero_area, T* cp = nullptr, T* nn_out = nullptr) {
     if (!zero_area) {
         const T abx = bx - ax, aby = by - ay, abz = bz - az;
         const T acx = cx - ax, acy = cy - ay, acz = cz - az;
         const T nx = aby * acz - abz * acy, ny = abz * acx - abx * acz, nz = abx * acy - aby * acx;
         const T nn = nx * nx + ny * ny + nz * nz;
+        if (nn_out) *nn_out = nn;
         const T apx = px - ax, apy = py - ay, apz = pz - az;
         const T bpx = px - bx, bpy = py - by, bpz = pz - bz;
         const T cpx = px - cx, cpy = py - cy, cpz = pz - cz;
@@ -161,7 +171,15 @@ meshsdf_slab_kernel(const float* __restrict__ verts, const int32_t* __restrict__
     float px = 0.f, py = 0.f, pz = 0.f;
     if (i < Q) { px = query[3 * i]; py = query[3 * i + 1]; pz = query[3 * i + 2]; }
     const double qx = px, qy = py, qz = pz;
-    const float eps = kEpsScale * (fmaxf(fabsf(px), fmaxf(fabsf(py), fabsf(pz))) + vmax);
+    // the fp32 pass in units of 2^e (above): s = 2^-e, e clamped so that s is a normal number
+    const float pmax = fmaxf(fabsf(px), fmaxf(fabsf(py), fabsf(pz)));
+    int e = 0;
+    if (isfinite(pmax)) frexpf(fmaxf(pmax, vmax), &e);
+    e = max(-126, min(126, e));
+    const float s = __int_as_float((127 - e) << 23);
+    const double s2 = (double)s * s;
+    const float spx = px * s, spy = py * s, spz = pz * s;
+    const float eps = kEpsScale * (pmax * s + vmax * s);
     float best32 = INFINITY, thr = INFINITY;
     double best64 = INFINITY, wind = 0.0;
     int32_t best_face = -1;
@@ -185,12 +203,17 @@ meshsdf_slab_kernel(const float* __restrict__ verts, const int32_t* __restrict__
             const float cx = sv[6][k], cy = sv[7][k], cz = sv[8][k];
             const bool zero = fl & kZeroArea;
             float d2f = 0.f;
-            const bool force = fl & kForce64;
-            if (!force) d2f = tri_dist2<float>(px, py, pz, ax, ay, az, bx, by, bz, cx, cy, cz, false);
+            bool force = fl & kForce64;
+            if (!force) {
+                float nn;
+                d2f = tri_dist2<float>(spx, spy, spz, ax * s, ay * s, az * s, bx * s, by * s, bz * s, cx * s, cy * s,
+                                       cz * s, false, nullptr, &nn);
+                force = !(nn >= kMinNN);
+            }
             if (force || d2f <= thr) {
                 const double d2 = tri_dist2<double>(qx, qy, qz, ax, ay, az, bx, by, bz, cx, cy, cz, zero);
                 if (d2 < best64) { best64 = d2; best_face = (int32_t)(t + k); }
-                if (force) d2f = (float)d2;
+                if (force) d2f = (float)(d2 * s2);
                 if (d2f < best32) {
                     best32 = d2f;
                     thr = best32 + kRelTol * best32 + 2.f * sqrtf(best32) * eps + eps * eps;
